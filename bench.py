@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- frames/sec of the OpenSora-v1.2 denoising loop on the vsb200 sm_100a path (driver contract).
+"""bench.py -- frames/sec of the OpenSora-v1.2 denoising loop on the vsb200 sm_90a path.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload NAME] [--pab]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload NAME] [--pab] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" is one iteration of the RFLOW sampling loop (schedulers/scheduling_rflow_open_sora.py:238-250 in the
@@ -18,6 +18,10 @@ other kernels), cpu_baseline (the oracle port on the host cores, bounded sample,
 the reference's eager path = the oracle restatement on torch/cuBLAS/SDPA library kernels on the same GPU), dsp_parity
 (N > 1: sharded == unsharded, bit for bit, before anything is timed), clocks, gpu_launches.
 --impl reference times the reference's CPU path (oracle port).
+--dump-outputs DIR (--impl ours) writes the latents the timed path produced in its last step (resident arm: latents.npy;
+host-buffer arm: latents_e2e.npy) as float32 .npy files.  --impl reference times a bounded sample of single blocks, which
+produces no denoising step to dump, so the two options are rejected together.  Weights and inputs are seeded, so two builds run with the same arguments
+can be compared output for output.
 """
 import argparse
 import json
@@ -52,9 +56,22 @@ def _peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return dict(tflops=d.get("bf16_tflops_sustained", 1386.7), tflops_burst=d.get("bf16_tflops", 1674.1),
-                    hbm=d.get("hbm_gbs", 6572.9), src="measured (MEASURED_PEAKS.json, sustained bf16 GEMM)")
-    return dict(tflops=1400.0, tflops_burst=1590.0, hbm=6650.0, src="fallback (B200_PROFILING.md)")
+        return dict(tflops=d.get("bf16_tflops_sustained", 989.0), tflops_burst=d.get("bf16_tflops", 989.0),
+                    hbm=d.get("hbm_gbs", 3350.0), src="measured (MEASURED_PEAKS.json, sustained bf16 GEMM)")
+    # NVIDIA H100 SXM data sheet (700 W): dense BF16 989 TFLOP/s, HBM3 3.35 TB/s -- a bound, not a measured rate
+    return dict(tflops=989.0, tflops_burst=989.0, hbm=3350.0, src="H100 SXM data sheet (dense BF16, 700 W)")
+
+
+def dump_outputs(args, **arrays):
+    """--dump-outputs DIR: each tensor as DIR/<name>.npy in float32."""
+    if not args.dump_outputs:
+        return
+    import numpy as np
+
+    os.makedirs(args.dump_outputs, exist_ok=True)
+    torch.cuda.synchronize()
+    for name, t in arrays.items():
+        np.save(os.path.join(args.dump_outputs, name + ".npy"), t.detach().float().cpu().numpy())
 
 
 def step_flops(W, depth=28, C=1152, B=2):
@@ -212,8 +229,8 @@ def run_reference(args):
         "cpu_baseline": {"value": val, "unit": "frames/s", "cores": cores, "kind": "port", "sample": desc,
                          "step_seconds_extrapolated": spread,
                          "note": "ms_per_step is EXTRAPOLATED from the bounded sample (the full step would take hours on the "
-                                 "host cores); /root/reference itself cannot travel to the GPU box, the port is pinned "
-                                 "bit-exact to it by tests/test_oracle_vs_reference.py"},
+                                 "host cores); the port is pinned bit-exact to the reference by "
+                                 "tests/test_oracle_vs_reference.py and the golden outputs under tests/golden/"},
         "e2e": {"value": val, "unit": "frames/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
     }
     print(json.dumps(line), flush=True)
@@ -224,7 +241,7 @@ def _config(args, W):
             "sampling_steps": W["steps"], "latent": list(W["lat"]), "cfg_batch": 2, "text_tokens": W["L"],
             "architecture": "STDiT3-XL/2 (hidden 1152, 16 heads x 72, 28+28 blocks)", "pab": bool(args.pab),
             "parallelism": f"dsp{args.gpus}" if args.gpus > 1 else "single",
-            "l2": "per-step working set (activations 332 MB/tensor at 720p) exceeds the 126 MB L2; no flush needed"}
+            "l2": "per-step working set (activations 332 MB/tensor at 720p) exceeds the 50 MB L2; no flush needed"}
 
 
 def make_line(args, W, world, sec, sec_e2e, sec_profiled, launches, roofline, shares, cpu_base, clocks, peaks, depth,
@@ -458,6 +475,8 @@ def run_ours(args):
     # our launches inside the two timed regions: host launches + the launches baked into every replayed graph
     launches = ((kernels.launch_count() - l0) + (stepper.replayed_launches - r0)) // 2
     clocks = sampler.stop()
+    if rank == 0:
+        dump_outputs(args, latents=state["z"], latents_e2e=out_host)
 
     # ---- per-kernel pass: EAGER steps with CUDA-event pairs around every launch of ours (not part of value) ----
     eager = StepGraph(net, 7.0, enabled=False)
@@ -486,10 +505,7 @@ def run_ours(args):
     gm = by_kind.get("gemm", [1e-9, 0.0, 1])
     gemm_tflops = gm[1] / (gm[0] * 1e-3) / 1e12
     traffic = None
-    tpath = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    if os.path.exists(tpath) and args.workload == "opensora_720p_68f_50step":
-        traffic = json.load(open(tpath)).get("gemm_720p_n1")
-    roofline = {"kernel": "gemm2_bf16_tn_kernel / gemm_bf16_tn_kernel (every Linear layer of the step)",
+    roofline = {"kernel": "gemm_wgmma_kernel (every Linear layer of the step)",
                 "bound": "tensor", "achieved": gemm_tflops,
                 "peak": peaks["tflops"], "unit": "TFLOP/s", "frac": gemm_tflops / peaks["tflops"], "traffic": traffic,
                 "peak_source": peaks["src"], "launches_timed": gm[2],
@@ -701,6 +717,8 @@ def run_cogvideox(args):
     net.reset_pab_state()
     sec_e2e = timed(step_e2e, args.steps)
     clocks = sampler.stop()
+    if rank == 0:
+        dump_outputs(args, latents=state["z"], latents_e2e=out_host)
     net.reset_pab_state()
     kernels.PROFILE, kernels.PROFILE_KINDS = [], None
     sec_prof = timed(step_resident, args.steps)
@@ -727,7 +745,7 @@ def run_cogvideox(args):
                    "latent": list(W["lat"]), "cfg_batch": 2, "text_tokens": 226, "joint_sequence": 226 + 13 * 30 * 45,
                    "architecture": "CogVideoX-2B transformer (hidden 1920, 30 heads x 64, 30 blocks)", "pab": bool(args.pab),
                    "parallelism": par, "first_schedule_index": first,
-                   "l2": "per-step working set (136 MB per activation tensor, 30 blocks) exceeds the 126 MB L2; no flush needed"},
+                   "l2": "per-step working set (136 MB per activation tensor, 30 blocks) exceeds the 50 MB L2; no flush needed"},
         "e2e": {"value": W["frames"] / (W["steps"] * sec_e2e / args.steps), "unit": "frames/s",
                 "h2d_bytes_per_step": z_host.numel() * 4, "d2h_bytes_per_step": out_host.numel() * 4,
                 "ms_per_step": sec_e2e / args.steps * 1e3},
@@ -798,6 +816,7 @@ def _simple_bench(args, name, net, one, n_sched, z_host, dt, frames, steps, conf
     net.reset_pab_state()
     sec_e2e = timed(step_e2e, args.steps)
     clocks = sampler.stop()
+    dump_outputs(args, latents=state["z"], latents_e2e=out_host)
     net.reset_pab_state()
     kernels.PROFILE, kernels.PROFILE_KINDS = [], None
     sec_prof = timed(step_resident, args.steps)
@@ -885,10 +904,10 @@ def run_vchitect(args):
     config = {"resolution": "288x480", "frames": 40, "sampling_steps": 100, "latent": list(W["lat"]), "forwards_per_step": 2,
               "text_tokens": L, "tokens_per_frame": S + L,
               "architecture": "Vchitect-2.0-2B transformer (hidden 1536, 24 heads x 64, 24 MMDiT blocks)",
-              "l2": "per-step working set (107 MB per joint activation tensor, 24 blocks) exceeds what stays in the 126 MB L2 "
+              "l2": "per-step working set (107 MB per joint activation tensor, 24 blocks) exceeds what stays in the 50 MB L2 "
                     "across a block; no flush needed"}
     _simple_bench(args, "vchitect_2b_40f_288x480_100step", net, one, len(ts), z_host, dt, W["frames"], W["steps"], config, "gemm",
-                  "gemm2_bf16_tn_kernel / gemm_bf16_tn_kernel (every Linear of the two forwards)", "bf16",
+                  "gemm_wgmma_kernel (every Linear of the two forwards)", "bf16",
                   args.first_step if args.first_step >= 0 else (20 if args.pab else 0))
 
 
@@ -942,7 +961,7 @@ def run_osp_v120(args):
     config = {"resolution": "480x640", "frames": 29, "sampling_steps": 100, "latent": list(W["lat"]), "cfg_batch": 2,
               "text_tokens": W["text"][0], "tokens": W["lat"][1] * (W["sample_size"][0] // 2) * (W["sample_size"][1] // 2),
               "architecture": "OpenSoraT2V-ROPE-L/122 (hidden 2304, 24 heads x 96, 32 blocks, full 3-D attention)",
-              "l2": "per-step working set (88 MB per activation tensor, 32 blocks) exceeds what stays in the 126 MB L2 across a "
+              "l2": "per-step working set (88 MB per activation tensor, 32 blocks) exceeds what stays in the 50 MB L2 across a "
                     "block; no flush needed"}
     _simple_bench(args, "osp_v120_29f_480p_100step", net, one, len(ts), z_host, dt, W["frames"], W["steps"], config, "attn_flash",
                   "attn_mma_kernel<96> behind vsb_attn_flash (3-D self attention over 9600 tokens + text cross attention)", "f16",
@@ -965,7 +984,11 @@ def main():
     ap.add_argument("--no-graph", action="store_true", help="launch every kernel from the host instead of replaying CUDA graphs")
     ap.add_argument("--first-step", type=int, default=-1, help="schedule index of the first timed step (default 0; 22 with --pab: inside the broadcast range)")
     ap.add_argument("--opt", action="append", default=[], help="kernel selection knob name=value (vsb_set_option)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the latents of the last timed step as float32 .npy files into DIR (--impl ours)")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes the outputs of --impl ours; --impl reference times single-block samples only")
     if args.workload.startswith("cogvideox"):
         if args.impl == "reference":
             print(json.dumps({"impl": "reference", "unavailable": "the CPU reference arm is defined for the OpenSora workloads"}))

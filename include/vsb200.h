@@ -1,8 +1,8 @@
-/* vsb200.h -- C-ABI of libvsb200.so: the B200-native (sm_100a) kernels behind the VideoSys DiT denoising hot path.
+/* vsb200.h -- C-ABI of libvsb200.so: the H100-native (sm_90a) kernels behind the VideoSys DiT denoising hot path.
  *
  * The reference (NUS-HPC-AI-Lab/VideoSys @ 4cce4778) is pure Python and exposes no FFI/plugin boundary
  * (SURVEY.md section 8b); this header is the boundary a maintainer binds with ctypes (INTEGRATION.md shows the
- * stub).  Each entry cites the reference code it replaces (paths relative to /root/reference/videosys/).
+ * stub).  Each entry cites the reference code it replaces (paths relative to the reference's videosys/ package).
  *
  * Conventions
  *   - plain pointers and sizes; every pointer is DEVICE memory unless named host_*; bf16 = uint16 storage.
@@ -22,45 +22,27 @@ extern "C" {
 typedef enum {
   VSB_OK = 0,
   VSB_ERR_INVALID = -1,     /* bad argument (null pointer, non-positive size) */
-  VSB_ERR_UNSUPPORTED = -2, /* shape / alignment outside what the sm_100a kernels handle */
+  VSB_ERR_UNSUPPORTED = -2, /* shape / alignment outside what the sm_90a kernels handle */
   VSB_ERR_CUDA = -3,        /* CUDA runtime / driver error (text in vsb_last_error) */
-  VSB_ERR_NO_DEVICE = -4    /* no sm_100 device: the library never falls back to the CPU */
+  VSB_ERR_NO_DEVICE = -4    /* no sm_90 device: the library never falls back to the CPU */
 } vsb_status;
 
 typedef uint16_t vsb_bf16;
 
 int vsb_version(void);
 const char* vsb_last_error(void);
-/* Checks that `device` is compute capability 10.x and loads cuTensorMapEncodeTiled. */
+/* Checks that `device` is compute capability 9.0 and loads cuTensorMapEncodeTiled. */
 int vsb_init(int device);
 /* Number of kernels this library has launched since load (all entries); bench.py reports the delta. */
 unsigned long long vsb_launch_count(void);
 /* Encoded TMA tensor maps are cached by (base, shape, strides, box, swizzle): which = 0 -> hits, 1 -> misses (host
  * cuTensorMapEncodeTiled calls actually made).  Option "tmap_cache" (default 1) turns the cache off. */
 unsigned long long vsb_tmap_cache_stats(int which);
-/* Run-time kernel selection knobs (not a backend switch: every choice is an sm_100a kernel of this library).
- *   "gemm_2sm" (default 1): CTA-pair (tcgen05 cta_group::2, M = 256) GEMM for M >= 1024 when N % 192 == 0 or
- *   N % 256 == 0; 0 forces the single-CTA (M = 128) kernel everywhere. */
-int vsb_set_option(const char* name, int value);
-/*   "attn_variant" (default -1 = auto): schedule of vsb_attn_flash.  2 = 64-key tiles with a double-buffered S in TMEM
- *   and four MMA issuer warps, one CTA per pair of query tiles; 3 = the same tiles under persistent CTAs (one per SM,
- *   running ahead across query pairs; auto picks it for nk <= 1024, where per-CTA fixed costs dominate); 0 = 128-key
- *   tiles with the two softmax warpgroups ping-ponging (first version, kept for comparison).
- *   "attn_poly_exp" (default 0; variants 2, 3): 1 / 2 / 3 = 25 / 37.5 / 50 % of the exp2 as a polynomial on the FMA
- *   pipe (no gain measured at sustained clocks; kept as a knob).
- *   "attn_pingpong" (default 1, variant 0): the warpgroups alternate on the MUFU phase.
- *   Same results up to fp32 rounding.
- * vsb_debug_attn_trace: device buffer of 9*16*4 int64 that CTA (0,0,0) of vsb_attn_flash fills with clock64()
- * timestamps (profiling aid, NULL disables). */
-int vsb_debug_attn_trace(void* device_buffer);
-/*   "attn_variant" 4 = variant 2 with the query rows resident in TMEM (S = Q K^T issued as TS MMAs: the A operand no
- *   longer re-read from shared memory on every K step) and 8 instead of 6 K/V stages; 5 = 4 with the softmax row sum
- *   accumulated by the tensor core (ones written into the zero padding column d = 72 of every V tile; head_dim 72).
- *   6 = up to 320 keys (text cross-attention): K/V of a (batch, head) resident in shared memory, 160-key score tiles
- *   (auto for nk <= 320).
+/* Run-time kernel selection knobs (not a backend switch: every choice is an sm_90a kernel of this library).
  *   "dsp_rowwise" (default 1): vsb_dsp_scatter decodes indices once per token row; 0 = the first version (per vector).
  *   "ln_occupancy" (default 3): 4 = vsb_ln_modulate compiled for 4 resident blocks per SM (64 registers).
  *   "tmap_cache" (default 1): cache of encoded TMA tensor maps. */
+int vsb_set_option(const char* name, int value);
 
 /* ---- AdaLN: LayerNorm(eps, no affine) -> x*(1+scale)+shift with per-frame t / t0 select --------------------
  * replaces norm1/norm2 + t2i_modulate + t_mask_select: models/transformers/open_sora_transformer_3d.py:47-48,
@@ -152,9 +134,9 @@ int vsb_attn_short(const vsb_bf16* qkv, vsb_bf16* out, const vsb_bf16* wq, const
                    const float* rope_sin, int n_outer, int n_inner, long long outer_stride, long long inner_stride,
                    long long tok_stride, int n, int H, int D, float eps, float scale, int flags, void* stream);
 
-/* ---- GEMM on tcgen05: out[M,N] = act(A[M,K] @ W[N,K]^T + bias[N]) ---------------------------------------------
+/* ---- GEMM on wgmma: out[M,N] = act(A[M,K] @ W[N,K]^T + bias[N]) ---------------------------------------------
  * replaces every nn.Linear on the path (attentions.py:59,107,156-157; timm Mlp fc1/fc2) and the tanh-GELU between
- * fc1 and fc2 (models/modules/activations.py:3).  bf16 in, fp32 accumulate in TMEM, bf16 out.
+ * fc1 and fc2 (models/modules/activations.py:3).  bf16 in, fp32 accumulate in registers, bf16 out.
  *   act: 0 = none, 1 = gelu_tanh applied to bf16(acc+bias) (the eager rounding point).
  *   Requirements: K % 8 == 0, N % 8 == 0, 16-byte aligned pointers, row-major contiguous. */
 int vsb_gemm_bias_act(const vsb_bf16* A, const vsb_bf16* W, const vsb_bf16* bias, vsb_bf16* out, int M, int N, int K,
@@ -164,19 +146,18 @@ int vsb_gemm_bias_act(const vsb_bf16* A, const vsb_bf16* W, const vsb_bf16* bias
  *   y = bf16(A @ W^T + bias);  g = gate_row >= 0 ? bf16(gate * y) : y;  out = bf16(resid + g)
  * gate = mod[sel(b,t), b, gate_row, :] with the per-frame t/t0 select of x_mask (as in vsb_gate_residual); M == B*T*S.
  * replaces proj/fc2 Linear + open_sora_transformer_3d.py:219-228,:270-284 (gate_row 2 / 5) and cross proj + :240
- * (gate_row -1).  out may alias resid.  Returns 1 WITHOUT launching when the CTA-pair kernel does not take the shape
- * (M < 1024 or N not a multiple of 192/256): the caller then uses vsb_gemm_bias_act + vsb_gate_residual. */
+ * (gate_row -1).  out may alias resid.  Same requirements as vsb_gemm_bias_act. */
 int vsb_gemm_bias_residual(const vsb_bf16* A, const vsb_bf16* W, const vsb_bf16* bias, const vsb_bf16* resid,
                            vsb_bf16* out, const vsb_bf16* mod, const uint8_t* x_mask, int gate_row, int M, int N, int K,
                            int B, int T, int S, void* stream);
 
-/* ---- flash attention on tcgen05 (spatial self-attention and text cross-attention) -------------------------------
+/* ---- flash attention (spatial self-attention and text cross-attention) -------------------------------
  * replaces F.scaled_dot_product_attention at attentions.py:100 and :268 (bool key mask = per-batch key count).
  * q/k/v are strided views: element (b, n, h, d) at base + b*batch_stride + n*row_stride + h*D + d (strides in
  * elements, multiples of 8).  out [nb, nq, H*D] contiguous.  kv_lens (host int array, nullable) = valid keys per
- * batch (<= nk, nb <= 64 when given).  head_dim 72 / 64: the tcgen05 kernels; 96 (Open-Sora-Plan v1.2.0,
- * open_sora_plan_v120_transformer_3d.py:929-931), 128, 80, 48, 32: the same contract on the warp-level tensor path
- * (mma.sync, FlashAttention-2 schedule, csrc/attn_mma.cu). */
+ * batch (<= nk, nb <= 64 when given).  head_dim 64 / 72 run on the warpgroup tensor cores (TMA + wgmma,
+ * csrc/attn_wgmma.cu); 32, 48, 80, 96 (Open-Sora-Plan v1.2.0, open_sora_plan_v120_transformer_3d.py:929-931) and 128 on
+ * the warp-level tensor cores (mma.sync, FlashAttention-2 schedule, csrc/attn_mma.cu). */
 int vsb_attn_flash(const vsb_bf16* q, const vsb_bf16* k, const vsb_bf16* v, vsb_bf16* out, int nb, int nq, int nk,
                    int H, int D, long long q_row_stride, long long q_batch_stride, long long kv_row_stride,
                    long long kv_batch_stride, const int* host_kv_lens, float scale, void* stream);
@@ -232,7 +213,7 @@ int vsb_gate_residual_dsp(const vsb_bf16* x, void* const* host_peer_y, vsb_bf16*
 
 /* Symmetric receive windows for the reshard: cudaMalloc'ed (zeroed) here so that a CUDA IPC handle maps the exact
  * base address; handles (64 bytes) are exchanged once at initialize() over the process group's store.
- * replaces nothing in the reference (NCCL owns its buffers); this is the B200-native plumbing for P2P stores. */
+ * replaces nothing in the reference (NCCL owns its buffers); this is the native plumbing for P2P stores. */
 int vsb_dsp_alloc(void** out, size_t bytes);
 int vsb_dsp_free(void* p);
 int vsb_ipc_get_handle(void* devptr, void* out_handle64);

@@ -1,5 +1,5 @@
 """TEST INFRASTRUCTURE ONLY -- Open-Sora-Plan v1.1.0 parity cases shared by oracle/gen_golden_osp.py (which runs the
-UNMODIFIED reference model on them, authoring container) and tests/test_osp_gpu.py (which runs the B200 product on the same
+UNMODIFIED reference model on them, authoring container) and tests/test_osp_gpu.py (which runs the native product on the same
 seeded inputs and weights and compares with the stored reference outputs)."""
 import torch
 

@@ -1,13 +1,13 @@
 """TEST INFRASTRUCTURE ONLY -- loads the *unmodified* reference modules for oracle pinning.
 
-Imports VideoSys' OpenSora hot-path modules straight from ``/root/reference`` (read-only) by
+Imports VideoSys' OpenSora hot-path modules straight from the reference tree (``VSB_REFERENCE_ROOT``, read-only) by
 registering a bare ``videosys`` namespace package (skipping ``videosys/__init__.py:1-12`` which
 pulls every pipeline -> diffusers) and stubbing the third-party names that are not installed in
 this image (timm ``Mlp``/``DropPath``, colossalai ``ProcessGroupMesh``, diffusers ``Attention``,
 ``rotary_embedding_torch.RotaryEmbedding``, imageio, omegaconf).  Recipe: SURVEY.md Appendix C.
 
 Only ``tests/`` and ``oracle/gen_golden.py`` may import this file, and only inside the authoring
-container: ``/root/reference`` does not exist on the GPU box, ``available()`` says so.
+machine that has the reference tree; elsewhere ``available()`` says it is absent.
 """
 import importlib
 import os

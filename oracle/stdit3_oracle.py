@@ -8,12 +8,12 @@ Every function is a functional restatement (state_dict in, tensors out; no nn.Mo
 singletons) of the reference code it cites, keeping the reference's *op order and rounding points*:
 each eager op rounds to the storage dtype exactly where the reference's eager op does, so on CPU in
 the same dtype the two are bit-identical (pinned in tests/test_oracle_vs_reference.py, which runs
-wherever ``/root/reference`` exists, and by the committed golden vectors in tests/golden/).
+wherever the reference tree is available, and by the committed golden vectors in tests/golden/).
 
 Third-party pieces that are not in the reference tree and are restated from their published
 semantics (SURVEY.md section 8c): timm ``Mlp`` (fc2(act(fc1(x)))), ``rotary_embedding_torch``
 ``RotaryEmbedding.rotate_queries_or_keys`` (interleaved pairs, theta 1e4, fp32 math, cast back).
-Citations are relative to /root/reference/videosys/.
+Citations are relative to the reference's videosys/ package.
 """
 import math
 from typing import Dict, List, Optional

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""R-GPU-1 (BASELINE.md section 2): the reference's eager PyTorch path on ONE B200, i.e. the oracle's op-for-op
+"""R-GPU-1 (BASELINE.md section 2): the reference's eager PyTorch path on ONE GPU, i.e. the oracle's op-for-op
 restatement of STDiT3.forward executed with torch/cuBLAS/SDPA library kernels on the GPU.  Measurement
 infrastructure (lives under tests/ because it executes oracle/); never used by the product or by bench.py's value.
 
@@ -57,7 +57,7 @@ def main():
         e1.record()
         torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / args.steps
-    out = {"what": "reference eager path (oracle restatement on torch/cuBLAS/SDPA), 1x B200", "workload": args.workload,
+    out = {"what": "reference eager path (oracle restatement on torch/cuBLAS/SDPA), 1 GPU", "workload": args.workload,
            "ms_per_step": ms, "frames_per_s": W["frames"] / (W["steps"] * ms / 1e3), "steps_timed": args.steps,
            "torch": torch.__version__}
     print(json.dumps(out))

@@ -65,7 +65,11 @@ def gemm_bias_act(a, w, bias=None, act=0, out=None):
 
 
 def gemm_bias_residual(a, w, bias, resid, mod=None, x_mask_u8=None, gate_row=-1, B=1, T=1, S=1, out=None):
-    return None  # "shape not taken": the callers fall back to gemm_bias_act + gate_residual, like on small shapes
+    y = gemm_bias_act(a, w, bias).reshape(resid.shape)
+    out = resid if out is None else out
+    if gate_row >= 0:
+        return gate_residual(resid, y, mod, x_mask_u8, gate_row, B, T, S, out=out)
+    return residual_add(resid, y, out=out)
 
 
 def _rope(x, cos, sin, pos):

@@ -61,7 +61,7 @@ def test_product_does_not_import_the_oracle():
 
 
 def test_state_dict_is_reference_compatible():
-    """Key set and shapes of the B200 module == the reference STDiT3 (SURVEY.md Appendix D)."""
+    """Key set and shapes of the native module == the reference STDiT3 (SURVEY.md Appendix D)."""
     from videosys_b200.models.transformers.open_sora_transformer_3d import STDiT3, STDiT3Config
 
     cfg = cases.small_model_cfg(depth=2)
@@ -134,6 +134,7 @@ def test_pab_mlp_skip_spec():
 
 # ---- DSP comm over gloo, world_size 2 ------------------------------------------------------------------------
 def _dsp_worker(rank, world, port, T, S, q):
+    os.environ["CUDA_VISIBLE_DEVICES"] = ""  # a CPU test: gloo ranks, never NCCL on a shared local GPU
     os.environ["MASTER_ADDR"] = "127.0.0.1"
     os.environ["MASTER_PORT"] = str(port)
     try:
@@ -188,6 +189,7 @@ def test_dsp_comm_gloo_world2(T, S):
 
 
 def _ulysses_worker(rank, world, port, q):
+    os.environ["CUDA_VISIBLE_DEVICES"] = ""  # a CPU test: gloo ranks, never NCCL on a shared local GPU
     os.environ["MASTER_ADDR"] = "127.0.0.1"
     os.environ["MASTER_PORT"] = str(port)
     try:

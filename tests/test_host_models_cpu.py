@@ -98,6 +98,9 @@ def test_osp_v110_host_logic_vs_reference_golden(monkeypatch, golden_dir, name):
     x, enc, m, tt = OC.inputs(name, torch.float32)
     out = net.eval()(x, timestep=tt, all_timesteps=[900, 500], encoder_hidden_states=enc, encoder_attention_mask=m,
                      return_dict=False)[0]
+    if f"{name}.idx" in gold:  # large case: the golden file holds a fixed seeded sample of the output elements
+        assert list(out.shape) == gold[f"{name}.shape"]
+        out = out.flatten()[gold[f"{name}.idx"].long()]
     assert torch.allclose(out, gold[f"{name}.fp32"], rtol=1e-4, atol=1e-5), (out - gold[f"{name}.fp32"]).abs().max()
 
 
@@ -175,6 +178,7 @@ def _sp_worker(rank, world, port, which, enable_cp, q):
     import os
     import traceback
 
+    os.environ["CUDA_VISIBLE_DEVICES"] = ""  # a CPU test: gloo ranks, never NCCL on a shared local GPU
     os.environ["MASTER_ADDR"] = "127.0.0.1"
     os.environ["MASTER_PORT"] = str(port)
     try:

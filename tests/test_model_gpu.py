@@ -1,4 +1,4 @@
-"""STDiT3 on the sm_100a kernels (videosys_b200) against the oracle and the reference's golden vectors.
+"""STDiT3 on the sm_90a kernels (videosys_b200) against the oracle and the reference's golden vectors.
 
 End-to-end tolerance (SURVEY.md fact 11 / BASELINE.md section 4): rtol 1e-3 is below one bf16 ulp, and the
 reference in bf16 is itself only within that band of its own fp32 run on a few % of elements.  So:

@@ -74,6 +74,9 @@ def test_osp_v110_forward_vs_reference_golden(gold, name, dt, dn):
               attention_mask=torch.ones(x.shape[0], x.shape[2], x.shape[3], x.shape[4]), encoder_attention_mask=m,
               return_dict=False)[0].cpu()
     r32, r16 = gold[f"{name}.fp32"], gold[f"{name}.{dn}"]
+    if f"{name}.idx" in gold:  # large case: the golden file holds a fixed seeded sample of the output elements
+        assert list(out.shape) == gold[f"{name}.shape"]
+        out = out.flatten()[gold[f"{name}.idx"].long()]
     e_ours, e_ref = _rel(out, r32), _rel(r16, r32)
     print(f"[parity] osp v110 {name} {dn}: ours-vs-reference fp32 {e_ours:.3e}, reference {dn}-vs-fp32 {e_ref:.3e}, "
           f"bit-equal to the reference's {dn} output {(out == r16).float().mean().item()*100:.1f} %")
@@ -168,7 +171,7 @@ def _net12(name, dt):
                                                (2, 70, 100, 2, 128, [100, 1]),
                                                (2, 33, 65, 5, 32, None)])
 def test_attn_mma_kernel(nb, nq, nk, H, D, lens, dt):
-    """vsb_attn_flash for head dims without a tcgen05 layout (csrc/attn_mma.cu) against fp32 attention on the same 16-bit
+    """vsb_attn_flash (csrc/attn_mma.cu) at head dims beyond the STDiT3 / CogVideoX ones against fp32 attention on the same 16-bit
     inputs: packed qkv (self) or separate q / kv buffers (cross), strided views, per-batch key counts."""
     if not torch.cuda.is_available():
         pytest.skip("no CUDA device")

@@ -1,4 +1,4 @@
-"""vsb200: the VideoSys DiT denoising hot path, B200-native (sm_100a CUDA behind a C-ABI).
+"""vsb200: the VideoSys DiT denoising hot path, H100-native (sm_90a CUDA behind a C-ABI).
 
 Same top-level names as ``videosys/__init__.py:1-22`` for the paths in scope (OpenSora, CogVideoX, Latte, Vchitect, Open-Sora-Plan v1.1.0); see DESIGN.md.
 """

@@ -1,6 +1,6 @@
 """ctypes binding of libvsb200.so (the C-ABI declared in include/vsb200.h).
 
-The library is built in-tree by ``videosys_b200.csrc.build`` (nvcc, sm_100a).  There is no CPU path and
+The library is built in-tree by ``videosys_b200.csrc.build`` (nvcc, sm_90a).  There is no CPU path and
 no alternative backend: if the shared object is missing and cannot be built, importing the kernels fails.
 """
 import ctypes as C
@@ -18,7 +18,6 @@ SIGNATURES = {
     "vsb_init": (_i, [_i]),
     "vsb_launch_count": (C.c_ulonglong, []),
     "vsb_set_option": (_i, [C.c_char_p, _i]),
-    "vsb_debug_attn_trace": (_i, [_vp]),
     "vsb_ln_modulate": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _f, _vp]),
     "vsb_ln_modulate_affine": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _f, _vp]),
     "vsb_qk_layernorm": (_i, [_vp, _vp, _vp, _vp, _vp, _sz, _i, _i, _f, _vp]),

@@ -6,7 +6,7 @@ split/gather_from_second_dim :307-318), inference only (no autograd functions); 
 ``ulysses_gather_heads`` are CogVideoX's head-scatter exchange on the packed qkv (cogvideox_transformer_3d.py:44-165).
 
 Two transports for the dimension switch:
-  * ``DspP2P`` (B200 path): one sm_100a kernel stores every 16-byte vector straight into the destination rank's
+  * ``DspP2P`` (native path): one sm_90a kernel stores every 16-byte vector straight into the destination rank's
     receive window over NVLink (CUDA-IPC mapped peer memory), flags + a wait kernel order the streams; no staging
     copies, no NCCL launch (csrc/dsp_p2p.cu, C-ABI vsb_dsp_scatter / vsb_dsp_wait).
   * ``torch.distributed.all_to_all_single`` (NCCL on GPU, gloo on CPU for the host-logic tests): the fallback
@@ -142,7 +142,7 @@ def ulysses_gather_heads(o: torch.Tensor, n_text: int, process_group) -> torch.T
 class DspP2P:
     """Symmetric receive windows + flags for the P2P dimension switch (one instance per process / sp group).
 
-    ``switch(x, T, S, to_spatial_shard)`` is the B200 replacement of STDiT3Block.dynamic_switch
+    ``switch(x, T, S, to_spatial_shard)`` is the native replacement of STDiT3Block.dynamic_switch
     (open_sora_transformer_3d.py:288-315): x is the local [B, t, s, C] tensor, the result is a view of this rank's
     receive window in the new layout.  The two directions own separate windows and flag arrays; stream order plus
     the data dependencies of the block make one window per direction sufficient (see DESIGN.md section 5).

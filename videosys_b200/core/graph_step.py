@@ -2,7 +2,7 @@
 
 A step of ``RFLOW.sample`` (reference schedulers/scheduling_rflow_open_sora.py:238-250) is ~3500 kernel launches,
 each 2-3 us of host work: on 8 GPUs, where a step is ~65 ms of device time, the launch gaps were ~11 % of the step.
-The whole step -- CFG concat, STDiT3.forward (our sm_100a kernels, the DSP peer-store switches, the NCCL gather),
+The whole step -- CFG concat, STDiT3.forward (our sm_90a kernels, the DSP peer-store switches, the NCCL gather),
 guidance combine and Euler update -- is therefore captured ONCE per distinct control flow and replayed:
 
   * inputs live in static device buffers (latent z, timestep t, dt, the per-frame x_mask); everything else the

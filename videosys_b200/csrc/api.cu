@@ -8,13 +8,8 @@
 
 namespace vsbs {
 thread_local char g_err[512] = "";
-int g_opt_gemm_2sm = 1;       // CTA-pair GEMM for M >= 1024
-int g_opt_attn_variant = -1;  // -1 = auto
-int g_opt_attn_pingpong = 1;  // variant 0 only
-int g_opt_attn_poly = 0;      // variants 2-5: fraction of exp2 on the FMA pipe
 int g_opt_dsp_rowwise = 1;    // 0: the first (per-vector) reshard kernel
 int g_opt_ln_occupancy = 3;   // ln_modulate: resident 256-thread blocks per SM the kernel is compiled for (3 or 4)
-long long* g_attn_trace = nullptr;
 std::atomic<unsigned long long> g_launches{0};
 static EncodeTiledFn g_encode = nullptr;
 static int g_sms = 0;
@@ -26,7 +21,7 @@ int num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (g_sms <= 0) g_sms = 148;
+    if (g_sms <= 0) g_sms = 132;
   }
   return g_sms;
 }
@@ -43,8 +38,7 @@ static int load_encode() {
 }
 
 // ---- tensor-map cache ------------------------------------------------------------------------------------------
-// cuTensorMapEncodeTiled costs ~1-2 us of host time; a denoising step made ~1800 such calls (3 per GEMM, 6 per
-// attention launch).  torch's caching allocator hands the same addresses back every step, so (base, shape, strides,
+// cuTensorMapEncodeTiled costs ~1-2 us of host time; a denoising step makes hundreds of such calls (3 per GEMM).  torch's caching allocator hands the same addresses back every step, so (base, shape, strides,
 // box, swizzle) repeats: an encoded map is a pure function of that key.  Bounded: cleared when it reaches kTmapCacheMax.
 struct TmapKey {
   const void* base;
@@ -146,7 +140,8 @@ extern "C" int vsb_init(int device) {
   if (device < 0 || device >= n) return fail(VSB_ERR_INVALID, "device %d out of range (%d devices)", device, n);
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return fail(VSB_ERR_CUDA, "cudaGetDeviceProperties failed");
-  if (prop.major != 10) return fail(VSB_ERR_NO_DEVICE, "device %d is sm_%d%d; vsb200 kernels are sm_100a only", device, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0)
+    return fail(VSB_ERR_NO_DEVICE, "device %d is sm_%d%d; vsb200 kernels are sm_90a only", device, prop.major, prop.minor);
   // cuTensorMapEncodeTiled needs a current context on some device, not on `device`: the caller's current device is
   // left untouched (the first version called cudaSetDevice(device) and silently changed it)
   g_sms = prop.multiProcessorCount;
@@ -155,22 +150,6 @@ extern "C" int vsb_init(int device) {
 
 extern "C" int vsb_set_option(const char* name, int value) {
   if (!name) return fail(VSB_ERR_INVALID, "set_option: null name");
-  if (!strcmp(name, "gemm_2sm")) {
-    g_opt_gemm_2sm = value;
-    return VSB_OK;
-  }
-  if (!strcmp(name, "attn_poly_exp")) {
-    g_opt_attn_poly = value;
-    return VSB_OK;
-  }
-  if (!strcmp(name, "attn_pingpong")) {
-    g_opt_attn_pingpong = value;
-    return VSB_OK;
-  }
-  if (!strcmp(name, "attn_variant")) {
-    g_opt_attn_variant = value;
-    return VSB_OK;
-  }
   if (!strcmp(name, "tmap_cache")) {
     g_opt_tmap_cache = value;
     return VSB_OK;

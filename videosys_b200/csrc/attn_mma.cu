@@ -1,11 +1,7 @@
-// vsb200 -- flash attention for the head dims the tcgen05 kernels are not laid out for (any multiple of 16 up to 128 other
-// than 64 / 72; in practice head_dim 96 = Open-Sora-Plan v1.2.0, open_sora_plan_v120_transformer_3d.py:837-960).
-//
-// The tcgen05 kernels (attn_tcgen05*.cu) hard-wire the 64 (+16) column split of K / V, the TMEM column budget of two
-// double-buffered score tiles plus O and Q, and the ones-column trick of head_dim 72; a 96-wide variant needs its own TMEM
-// plan (DESIGN.md section 10).  Until then this kernel carries those shapes on the warp-level tensor path: same interface
-// (strided q / k / v views, per-batch key counts, strided output), same arithmetic contract (fp32 scores, softmax scale
-// folded into exp2, P rounded to the 16-bit dtype before P V, fp32 accumulation), FlashAttention-2 schedule:
+// vsb200 -- flash attention forward for the head dims that attn_wgmma.cu is not laid out for (96: Open-Sora-Plan v1.2.0;
+// also 32, 48, 80, 128), FlashAttention-2 schedule on the warp-level tensor cores; and the vsb_attn_flash entry points,
+// which send head_dim 64 / 72 to the warpgroup kernel.  Arithmetic contract (both kernels): fp32 scores, softmax scale folded
+// into exp2, P rounded to the 16-bit dtype before P V, fp32 accumulation.
 //
 //   CTA = 8 warps = 128 query rows of one (batch, head); a warp owns 16 rows (one m16 tile), its Q fragments live in registers.
 //   Loop over 64-key tiles: K / V tile -> shared memory (cp.async into two buffers: the next tile loads while this one is
@@ -13,11 +9,10 @@
 //   S = Q K^T (mma.sync m16n8k16, fp32), online softmax on the accumulator fragments (row max / sum across the 4 lanes of a
 //   row), P re-packed as A fragments, O += P V (V fragments by ldmatrix.x4.trans).  Rows beyond the sequence are zero (Q) or
 //   masked to -inf (keys); V rows beyond the key count are zero so that 0 * garbage cannot produce NaN.
-//
-// mma.sync reaches a fraction of the tcgen05 rate: this is the functional path for those shapes, not a roofline kernel.
 #include "attn_params.cuh"
 
 namespace vsb {
+
 
 __device__ __forceinline__ void mm_ldsm_x4(uint32_t (&r)[4], const void* p) {
   asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
@@ -214,8 +209,7 @@ static int launch_mma(const bf16* q, const bf16* k, const bf16* v, long long kv_
   return check_launch("attn_mma");
 }
 
-// attn_tcgen05.cu routes vsb_attn_flash[_strided] here for head dims other than 64 / 72.
-int attn_mma_launch(const bf16* q, const bf16* k, const bf16* v, long long kv_row_stride, long long kv_batch_stride,
+static int attn_mma_launch(const bf16* q, const bf16* k, const bf16* v, long long kv_row_stride, long long kv_batch_stride,
                     const AttnParams& prm, int D, cudaStream_t st) {
   switch (D) {
     case 96: return launch_mma<96>(q, k, v, kv_row_stride, kv_batch_stride, prm, st);
@@ -223,8 +217,56 @@ int attn_mma_launch(const bf16* q, const bf16* k, const bf16* v, long long kv_ro
     case 80: return launch_mma<80>(q, k, v, kv_row_stride, kv_batch_stride, prm, st);
     case 48: return launch_mma<48>(q, k, v, kv_row_stride, kv_batch_stride, prm, st);
     case 32: return launch_mma<32>(q, k, v, kv_row_stride, kv_batch_stride, prm, st);
-    default: return fail(VSB_ERR_UNSUPPORTED, "attn_flash: head_dim %d (72 and 64 on tcgen05; 32, 48, 80, 96, 128 on mma.sync)", D);
+    default: return fail(VSB_ERR_UNSUPPORTED, "attn_flash: head_dim %d (32, 48, 64, 72, 80, 96, 128)", D);
   }
 }
 
 }  // namespace vsb
+
+using namespace vsb;
+
+extern "C" int VSB_API(vsb_attn_flash)(const vsb_bf16* q, const vsb_bf16* k, const vsb_bf16* v, vsb_bf16* out, int nb, int nq,
+                              int nk, int H, int D, long long q_row_stride, long long q_batch_stride,
+                              long long kv_row_stride, long long kv_batch_stride, const int* host_kv_lens, float scale,
+                              void* stream) {
+  return VSB_API(vsb_attn_flash_strided)(q, k, v, out, nb, nq, nk, H, D, q_row_stride, q_batch_stride, kv_row_stride,
+                                kv_batch_stride, (long long)H * D, (long long)nq * H * D, host_kv_lens, scale, stream);
+}
+
+extern "C" int VSB_API(vsb_attn_flash_strided)(const vsb_bf16* q, const vsb_bf16* k, const vsb_bf16* v, vsb_bf16* out, int nb,
+                                      int nq, int nk, int H, int D, long long q_row_stride, long long q_batch_stride,
+                                      long long kv_row_stride, long long kv_batch_stride, long long out_row_stride,
+                                      long long out_batch_stride, const int* host_kv_lens, float scale, void* stream) {
+  if (!q || !k || !v || !out || nb <= 0 || nq <= 0 || nk <= 0 || H <= 0) return fail(VSB_ERR_INVALID, "attn_flash: bad args");
+  if ((out_row_stride % 8) || (out_batch_stride % 8) || out_row_stride < (long long)H * D)
+    return fail(VSB_ERR_UNSUPPORTED, "attn_flash: output strides must be multiples of 8 elements, rows >= H*D apart");
+  if ((q_row_stride % 8) || (q_batch_stride % 8) || (kv_row_stride % 8) || (kv_batch_stride % 8) || !aligned16(q) ||
+      !aligned16(k) || !aligned16(v) || !aligned16(out))
+    return fail(VSB_ERR_UNSUPPORTED, "attn_flash: strides must be multiples of 8 elements and pointers 16B-aligned");
+  if (host_kv_lens && nb > kAttnMaxLens)
+    return fail(VSB_ERR_UNSUPPORTED, "attn_flash: per-batch key lengths need nb <= %d", kAttnMaxLens);
+  if (nb > 65535 || H > 65535) return fail(VSB_ERR_UNSUPPORTED, "attn_flash: grid too large");
+  AttnParams prm;
+  prm.out = (bf16*)out;
+  prm.out_row_stride = out_row_stride;
+  prm.out_batch_stride = out_batch_stride;
+  prm.q_row_stride = q_row_stride;
+  prm.q_batch_stride = q_batch_stride;
+  prm.nb = nb;
+  prm.nq = nq;
+  prm.nk = nk;
+  prm.H = H;
+  prm.scale_log2 = scale * 1.4426950408889634f;
+  prm.has_lens = host_kv_lens ? 1 : 0;
+  for (int i = 0; i < kAttnMaxLens; ++i) prm.lens[i] = 0;
+  if (host_kv_lens)
+    for (int i = 0; i < nb; ++i) {
+      if (host_kv_lens[i] < 1 || host_kv_lens[i] > nk) return fail(VSB_ERR_INVALID, "attn_flash: kv_lens[%d]=%d", i, host_kv_lens[i]);
+      prm.lens[i] = host_kv_lens[i];
+    }
+  if (D == 64 || D == 72)
+    return attn_wgmma_launch((const bf16*)q, (const bf16*)k, (const bf16*)v, kv_row_stride, kv_batch_stride, prm, D,
+                             (cudaStream_t)stream);
+  return attn_mma_launch((const bf16*)q, (const bf16*)k, (const bf16*)v, kv_row_stride, kv_batch_stride, prm, D,
+                         (cudaStream_t)stream);
+}

@@ -1,37 +1,17 @@
-// vsb200 -- shared between the two flash-attention kernels (attn_tcgen05.cu: 128-key tiles with ping-pong;
-// attn_tcgen05_kt64.cu: 64-key tiles with double-buffered S).
+// vsb200 -- parameters shared by the two flash-attention kernels (attn_wgmma.cu: head_dim 64 / 72 on the warpgroup tensor
+// cores; attn_mma.cu: the other head dims on mma.sync) and the vsb_attn_flash entry that dispatches between them.
 #pragma once
 #include "vsb_common.cuh"
 #include "vsb_host.h"
 
 namespace vsb {
 
-// Debug timeline: when AttnParams::trace != nullptr, CTA (0,0,0) records clock64() at [actor][tile < 16][event < 4]
-// (actor 0 = MMA thread, 1/2 = softmax warpgroup A/B, lane 0 of its first warp).  Null in normal runs.
-#define VSB_TRACE(actor, tile, ev)                                                                   \
-  do {                                                                                               \
-    if (p.trace != nullptr && (tile) < 16 && lane == 0 && (warp == 1 || (warp & 3) == 0) &&         \
-        blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0)                                       \
-      p.trace[((actor) * 16 + (tile)) * 4 + (ev)] = clock64();                                       \
-  } while (0)
-
-// per-warp variant (attn_tcgen05_kt64.cu): actor 0 = MMA issuer warps 0..3, 1..8 = softmax warps 4..11; 9*16*4 int64
-#define VSB_TRACE_W(tile, ev)                                                                            \
-  do {                                                                                                   \
-    if (p.trace != nullptr && (tile) < 16 && lane == 0 && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0) \
-      p.trace[((warp < 4 ? 0 : warp - 3) * 16 + (tile)) * 4 + (ev)] = clock64();                        \
-  } while (0)
-
 constexpr int kAttnMaxLens = 64;  // per-batch key counts travel by value in the kernel parameters
 struct AttnParams {
-  int poly_exp;  // host-side selector of the kt64 kernels' kPoly template (0 / 1 / 2 / 3 = 0 / 25 / 37.5 / 50 % of exp2 on the FMA pipe)
-  int pingpong;  // 128-key kernel only: 1 = the two softmax warpgroups take turns on the exp2 (MUFU) phase through named barriers
-  long long* trace;
   bf16* out;
   // out element (b, n, h, d) at out + b*out_batch_stride + n*out_row_stride + h*D + d (elements): the temporal
   // (T >= 30) path writes straight back into the token-major activation
   long long out_row_stride, out_batch_stride;
-  const bf16* q;  // raw query pointer + strides (elements): the Q-in-TMEM schedule moves its rows itself
   long long q_row_stride, q_batch_stride;
   int nb, nq, nk, H;
   float scale_log2;  // softmax scale * log2(e)
@@ -39,16 +19,9 @@ struct AttnParams {
   int lens[kAttnMaxLens];
 };
 
-
-// attn_tcgen05_kt64.cu.  tm = {q64, q16, k64, k16, v64, v16} with 64-row key boxes.
-// q_tmem: Q rows resident in TMEM, S = Q K^T issued as TS MMAs (attn_variant 4)
-int attn_flash_kt64_launch(const CUtensorMap* tm, const AttnParams& prm, int D, int poly, int q_tmem, cudaStream_t st);
-// attn_tcgen05_kvres.cu: nk <= 320, K/V resident in shared memory, 160-key score tiles.  tm key boxes have 160 rows.
-int attn_flash_kvres_launch(const CUtensorMap* tm, const AttnParams& prm, int D, cudaStream_t st);
-// attn_mma.cu: head dims other than 64 / 72 (96 = Open-Sora-Plan v1.2.0) on the warp-level tensor path; raw strided pointers.
-int attn_mma_launch(const bf16* q, const bf16* k, const bf16* v, long long kv_row_stride, long long kv_batch_stride,
-                    const AttnParams& prm, int D, cudaStream_t st);
-// attn_tcgen05_kt64p.cu: the same tiles under persistent CTAs.
-int attn_flash_kt64p_launch(const CUtensorMap* tm, const AttnParams& prm, int D, int poly, cudaStream_t st);
+// attn_wgmma.cu: head_dim 64 / 72; q / k / v are strided views (element (b, n, h, d) at base + b*batch_stride +
+// n*row_stride + h*D + d, strides in elements).
+int attn_wgmma_launch(const bf16* q, const bf16* k, const bf16* v, long long kv_row_stride, long long kv_batch_stride,
+                      const AttnParams& prm, int D, cudaStream_t st);
 
 }  // namespace vsb

@@ -8,10 +8,9 @@
 //   2. RMSNorm (+ RoPE from a per-block smem table, q scale) in place on q and k, three lanes per row;
 //   3. S = Q K^T and O = P V on the warp-level tensor path (mma.sync m16n8k16 / m16n8k8 bf16, fp32 accumulate,
 //      ldmatrix fragments; P is re-packed from the S accumulators, FA2 style) -- the sequences are far too short for
-//      a tcgen05 tile (20 keys against a 128-key MMA would waste 84 % of the work);
+//      a warpgroup MMA tile (20 keys against a 64-row x 128-key tile would waste most of the work);
 //   4. O staged over the dead Q rows and written by one TMA box store.
-// (The first version staged with per-lane 16-byte loads / stores: 4800 instructions per item, half of them index
-// arithmetic, 12 warps per SM: 1.08 ms for the 720p launch, 15 % of HBM peak -- profiles/r01_attn_short_ncu_full.txt.)
+// (Staging with per-lane 16-byte loads / stores instead costs 4800 instructions per item, half of them index arithmetic.)
 // Rounding follows the reference's eager op order (attentions.py:111-120): bf16(q*scale), bf16(q@k^T),
 // fp32 softmax, bf16(probs), bf16(probs@v).
 #include <type_traits>

@@ -1,4 +1,4 @@
-"""Builds libvsb200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Builds libvsb200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
     python -m videosys_b200.csrc.build [--force] [--verbose]
 """
@@ -7,14 +7,14 @@ import subprocess
 import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-SOURCES = ["api.cu", "elementwise.cu", "attn_short.cu", "gemm_tcgen05.cu", "gemm_tcgen05_2sm.cu", "attn_tcgen05.cu", "attn_tcgen05_kt64.cu", "attn_tcgen05_kt64p.cu", "attn_tcgen05_kvres.cu", "attn_mma.cu", "dsp_p2p.cu", "patch_embed.cu"]
+SOURCES = ["api.cu", "elementwise.cu", "attn_short.cu", "gemm_wgmma.cu", "attn_wgmma.cu", "attn_mma.cu", "dsp_p2p.cu", "patch_embed.cu"]
 # every kernel file below is compiled twice: bf16 (as is) and IEEE fp16 (-DVSB_HALF -> *.f16.o, entries suffixed _f16)
-TWINNED = ["elementwise.cu", "attn_short.cu", "gemm_tcgen05.cu", "gemm_tcgen05_2sm.cu", "attn_tcgen05.cu", "attn_tcgen05_kt64.cu", "attn_tcgen05_kt64p.cu", "attn_tcgen05_kvres.cu", "attn_mma.cu", "patch_embed.cu"]
-HEADERS = ["vsb_common.cuh", "vsb_host.h", "attn_params.cuh", "dsp_common.cuh", os.path.join("..", "..", "include", "vsb200.h")]
+TWINNED = ["elementwise.cu", "attn_short.cu", "gemm_wgmma.cu", "attn_wgmma.cu", "attn_mma.cu", "patch_embed.cu"]
+HEADERS = ["vsb_common.cuh", "vsb_host.h", "wgmma.cuh", "attn_params.cuh", "dsp_common.cuh", os.path.join("..", "..", "include", "vsb200.h")]
 LIB = os.path.join(HERE, "libvsb200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v",
 ]
 
@@ -23,7 +23,8 @@ def _stale(obj, src):
     if not os.path.exists(obj):
         return True
     t = os.path.getmtime(obj)
-    deps = [src] + [os.path.join(HERE, h) for h in HEADERS]
+    # this file too: a change of FLAGS (the target architecture) must rebuild every object
+    deps = [src, os.path.abspath(__file__)] + [os.path.join(HERE, h) for h in HEADERS]
     return any(os.path.getmtime(d) > t for d in deps)
 
 

@@ -6,7 +6,7 @@
 // Replaces open_sora_transformer_3d.py:568-572 (x_embedder -> rearrange -> + pos_emb -> rearrange) and :577
 // (split_sequence along S): the eager chain runs a cuDNN implicit GEMM with K = 16 plus two layout transposes, a
 // transposed read-modify-write for the position add and a slicing copy, all on the FULL sequence on every rank --
-// 1.6 ms per forward at 720p (profiles/r02_launches_720p_depth2.txt), which no longer shrinks with the number of GPUs.
+// and that cost does not shrink with the number of GPUs.
 //
 // Mapping: a thread owns 8 consecutive output channels (one 16-byte store per token) and keeps their 16 x 8 weights in
 // registers as fp32 for the whole kernel; a CTA walks tiles of 32 tokens whose 16 taps are staged in shared memory

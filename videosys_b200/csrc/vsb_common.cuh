@@ -1,4 +1,4 @@
-// vsb200 -- shared device helpers: PTX wrappers for mbarrier / TMA / tcgen05 / TMEM (sm_100a only).
+// vsb200 -- shared device helpers: PTX wrappers for mbarrier / TMA / wgmma (sm_90a).
 // No CUTLASS: every instruction the kernels rely on is spelled out here.
 #pragma once
 #include <cuda.h>
@@ -7,10 +7,6 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
-
-#if !defined(__CUDA_ARCH__) || (__CUDA_ARCH__ >= 1000)
-#define VSB_SM100 1
-#endif
 
 // ---- element type of this translation unit -------------------------------------------------------------------------
 // Every kernel file is compiled twice: as is (bf16: OpenSora, CogVideoX-5b) and with -DVSB_HALF (IEEE fp16: the dtype the
@@ -39,7 +35,6 @@ __device__ __forceinline__ float2 e2_to_float2(elem2 v) { return __half22float2(
 __device__ __forceinline__ elem2 floats_to_e2(float lo, float hi) { return __floats2half2_rn(lo, hi); }
 __device__ __forceinline__ bf16 float_to_e(float x) { return __float2half_rn(x); }
 __device__ __forceinline__ float e_to_float(bf16 x) { return __half2float(x); }
-constexpr uint32_t kUmmaFmtBits = 0u;  // a_format = b_format = F16
 #else
 typedef __nv_bfloat16 bf16;
 typedef __nv_bfloat162 elem2;
@@ -47,7 +42,6 @@ __device__ __forceinline__ float2 e2_to_float2(elem2 v) { return __bfloat1622flo
 __device__ __forceinline__ elem2 floats_to_e2(float lo, float hi) { return __floats2bfloat162_rn(lo, hi); }
 __device__ __forceinline__ bf16 float_to_e(float x) { return __float2bfloat16_rn(x); }
 __device__ __forceinline__ float e_to_float(bf16 x) { return __bfloat162float(x); }
-constexpr uint32_t kUmmaFmtBits = (1u << 7) | (1u << 10);  // a_format = b_format = BF16
 #endif
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
@@ -85,12 +79,6 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
-// remote arrive on the barrier at the same smem offset in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
-  uint32_t remote;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(cta));
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
-}
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
   asm volatile(
@@ -118,6 +106,15 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     }
   }
 }
+// Same watchdog without the printf: a function call between wgmma.mma_async and its wait makes ptxas serialize the
+// warpgroup MMAs, so the GEMM consumers wait with this one.
+__device__ __forceinline__ void mbar_wait_quiet(uint64_t* bar, uint32_t parity) {
+  if (mbar_try_wait(bar, parity)) return;
+  long long t0 = clock64();
+  while (!mbar_try_wait(bar, parity)) {
+    if (clock64() - t0 > VSB_WATCHDOG_CYCLES) __trap();
+  }
+}
 
 // ------------------------------------------------------------------------------------------
 // TMA (cp.async.bulk.tensor)
@@ -138,16 +135,6 @@ __device__ __forceinline__ void tma_load_4d(const CUtensorMap* m, uint64_t* bar,
       "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], "
       "[%2];" ::"r"(smem_u32(dst)),
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-// 2-SM variant: executed by both CTAs of a pair; the transaction bytes land on the LEADER's barrier
-// (peer bit cleared), data lands in the issuing CTA's smem.
-__device__ __forceinline__ void tma_load_2d_2sm(const CUtensorMap* m, uint64_t* bar, void* dst, int c0, int c1) {
-  uint32_t b = smem_u32(bar) & 0xFEFFFFFFu;
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, "
-      "%4}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(b), "r"(c0), "r"(c1)
       : "memory");
 }
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* src, int c0, int c1) {
@@ -176,254 +163,27 @@ __device__ __forceinline__ void tma_store_wait_read0() { asm volatile("cp.async.
 __device__ __forceinline__ void tma_store_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 // ------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
+// wgmma (warpgroup MMA): operands in shared memory, fp32 accumulators in registers; wrappers in wgmma.cuh
 // ------------------------------------------------------------------------------------------
-template <int kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst) {  // one full warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int kPending>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(kPending) : "memory");
 }
-template <int kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {  // same warp that allocated
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
+// Shared-memory matrix descriptor of a K-major tile written by TMA with SWIZZLE_128B: rows of 128 bytes (64 16-bit
+// elements), 8-row groups 1024 bytes apart (stride byte offset), leading byte offset unused, layout 1 = 128B swizzle.
+// Advancing K by 16 elements inside the swizzle atom adds 32 bytes to the start address.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t saddr) {
+  return uint64_t((saddr >> 4) & 0x3FFF) | (uint64_t(1) << 16) | (uint64_t(1024 >> 4) << 32) | (uint64_t(1) << 62);
 }
-template <int kCols>
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* smem_dst) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <int kCols>
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]; single issuing thread.
-__device__ __forceinline__ void umma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                        uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// A from TMEM (K-major by construction), B from smem.
-__device__ __forceinline__ void umma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                        uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_ss_2sm(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// commit: the mbarrier gets one arrival when all previously issued MMAs of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void umma_commit_2sm_mcast(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(cta_mask)
-      : "memory");
-}
-
-// ---- warp-converged issue helpers -------------------------------------------------------------------------------
-// tcgen05.mma / tcgen05.commit / TMA take their operands from UNIFORM registers.  Issued from inside `if (lane == 0)`
-// (divergent control flow) ptxas has to build every operand in vector registers and move it over with an
-// ELECT + R2UR.BROADCAST loop: ~20 dependent instructions (~80 cycles) per MMA, which starves the tensor pipe
-// (measured: 83 cycles per issued MMA).  These variants are executed by the WHOLE converged warp on warp-uniform
-// operands; `elected` (from elect_one()) predicates the single issuing lane inside the asm block.
-__device__ __forceinline__ uint32_t elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred;
-}
-__device__ __forceinline__ uint64_t desc_pack(uint32_t lo, uint32_t hi) {
-  uint64_t d;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(d) : "r"(lo), "r"(hi));
-  return d;
-}
-// high word of a shared-memory matrix descriptor: SBO (16-byte units) | version 1 | layout; low word = addr>>4 | LBO<<16
-__host__ __device__ constexpr uint32_t umma_desc_hi(uint32_t sbo_bytes, uint32_t layout) {
-  return ((sbo_bytes >> 4) & 0x3FFF) | (1u << 14) | (layout << 29);
-}
-__device__ __forceinline__ uint32_t umma_desc_lo(uint32_t saddr, uint32_t lbo_bytes) {
-  return ((saddr >> 4) & 0x3FFF) | (((lbo_bytes >> 4) & 0x3FFF) << 16);
-}
-__device__ __forceinline__ void umma_ss_w(uint32_t elected, uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                          uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p, pe;\n\tsetp.ne.b32 pe, %5, 0;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate), "r"(elected)
-      : "memory");
-}
-__device__ __forceinline__ void umma_ts_w(uint32_t elected, uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc,
-                                          uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p, pe;\n\tsetp.ne.b32 pe, %5, 0;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate), "r"(elected)
-      : "memory");
-}
-__device__ __forceinline__ void umma_ss_2sm_w(uint32_t elected, uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                              uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p, pe;\n\tsetp.ne.b32 pe, %5, 0;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "@pe tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate), "r"(elected)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_w(uint32_t elected, uint64_t* bar) {
-  asm volatile(
-      "{\n\t.reg .pred pe;\n\tsetp.ne.b32 pe, %1, 0;\n\t"
-      "@pe tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}" ::"r"(smem_u32(bar)),
-      "r"(elected)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_2sm_mcast_w(uint32_t elected, uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "{\n\t.reg .pred pe;\n\tsetp.ne.b32 pe, %2, 0;\n\t"
-      "@pe tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n\t}" ::"r"(
-          smem_u32(bar)),
-      "h"(cta_mask), "r"(elected)
-      : "memory");
-}
-
-__device__ __forceinline__ void mbar_arrive_expect_tx_w(uint32_t elected, uint64_t* bar, uint32_t bytes) {
-  asm volatile(
-      "{\n\t.reg .pred pe;\n\tsetp.ne.b32 pe, %2, 0;\n\t"
-      "@pe mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n\t}" ::"r"(smem_u32(bar)),
-      "r"(bytes), "r"(elected)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_w(uint32_t elected, const CUtensorMap* m, uint64_t* bar, void* dst, int c0,
-                                              int c1) {
-  asm volatile(
-      "{\n\t.reg .pred pe;\n\tsetp.ne.b32 pe, %5, 0;\n\t"
-      "@pe cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];\n\t}" ::"r"(
-          smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(elected)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_2sm_to_w(uint32_t elected, const CUtensorMap* m, uint32_t bar_cluster_addr,
-                                                     void* dst, int c0, int c1) {
-  asm volatile(
-      "{\n\t.reg .pred pe;\n\tsetp.ne.b32 pe, %5, 0;\n\t"
-      "@pe cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, "
-      "%4}], [%2];\n\t}" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(elected)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_w(uint32_t elected, const CUtensorMap* m, uint64_t* bar, void* dst, int c0,
-                                              int c1, int c2, int c3) {
-  asm volatile(
-      "{\n\t.reg .pred pe;\n\tsetp.ne.b32 pe, %7, 0;\n\t"
-      "@pe cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], "
-      "[%2];\n\t}" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(elected)
-      : "memory");
-}
-
-// Instruction descriptor, kind::f16, bf16 x bf16 -> fp32 (cute/arch/mma_sm100_desc.hpp InstrDescriptor bit layout).
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4)                      // c_format = F32
-         | kUmmaFmtBits                 // a_format = b_format = BF16 (F16 in the fp16 twin)
-         | (uint32_t(a_mn_major) << 15) | (uint32_t(b_mn_major) << 16) | (uint32_t(N >> 3) << 17) |
-         (uint32_t(M >> 4) << 24);
-}
-// Shared-memory matrix descriptor (SmemDescriptor bit layout): version=1 (sm100), LBO/SBO in 16-byte units.
-enum : uint64_t { kSwz128 = 2, kSwz64 = 4, kSwz32 = 6 };
-__device__ __forceinline__ uint64_t umma_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                                   uint64_t layout) {
-  return uint64_t((saddr >> 4) & 0x3FFF) | (uint64_t((lbo_bytes >> 4) & 0x3FFF) << 16) |
-         (uint64_t((sbo_bytes >> 4) & 0x3FFF) << 32) | (1ull << 46) | (layout << 61);
-}
-
-// TMEM -> registers: warp w may only touch lanes 32*(w%4) .. +31; thread t gets lane base+t, regs = columns.
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,"
-      "%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t (&r)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(
-          taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t (&r)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(taddr), "r"(r[0]),
-               "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-
-// ---- thread-block cluster helpers (CTA pairs for cta_group::2) ----
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of `p` (an address in MY shared memory) as seen in CTA `cta` of the cluster
-__device__ __forceinline__ uint32_t mapa_u32(const void* p, uint32_t cta) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_u32(p)), "r"(cta));
-  return r;
-}
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// 2-SM TMA load: data into MY smem, transaction bytes onto the barrier at cluster address `bar_cluster_addr`
-__device__ __forceinline__ void tma_load_2d_2sm_to(const CUtensorMap* m, uint32_t bar_cluster_addr, void* dst, int c0,
-                                                   int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, "
-      "%4}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1)
-      : "memory");
+// General form: leading / stride byte offsets and layout (1 = 128B, 2 = 64B, 3 = 32B swizzle).  For a K-major tile the stride
+// byte offset is the distance between 8-row groups; for an MN-major tile (rows along K, the N extent contiguous inside the
+// swizzle span) it is the distance between 8-row groups along K, and the leading byte offset the distance between swizzle
+// spans along N (unused when N fits in one span).
+__device__ __forceinline__ uint64_t wgmma_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo, uint32_t layout) {
+  return uint64_t((saddr >> 4) & 0x3FFF) | (uint64_t((lbo >> 4) & 0x3FFF) << 16) | (uint64_t((sbo >> 4) & 0x3FFF) << 32) |
+         (uint64_t(layout) << 62);
 }
 
 // named barrier among a subset of warps (ids 1..15; 0 is __syncthreads)
@@ -433,24 +193,6 @@ __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
 
 __device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-  float d;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
-}
-// 2^x on the FMA/ALU pipes (no MUFU): round-to-nearest split x = n + f, f in [-0.5, 0.5], degree-3 minimax
-// polynomial for 2^f (max relative error 7.5e-5, far below the bf16 rounding of P), exponent patched in with an
-// integer add.  Valid for x >= -126 (clamped); used for every other score so the MUFU pipe (the bound of the
-// attention kernel at head_dim 72) only sees half of the exponentials.
-__device__ __forceinline__ float exp2_poly(float x) {
-  x = fmaxf(x, -126.f);
-  const float t = x + 12582912.f;   // 1.5 * 2^23: rint(x) lands in the low mantissa bits
-  const float f = x - (t - 12582912.f);
-  float p = fmaf(f, 0.05517164245247841f, 0.2426111251115799f);
-  p = fmaf(f, p, 0.6932609677314758f);
-  p = fmaf(f, p, 0.9999280571937561f);
-  return __int_as_float(__float_as_int(p) + (__float_as_int(t) << 23));
 }
 __device__ __forceinline__ float fast_exp2(float x) {
   float y;

@@ -1,6 +1,6 @@
 """Thin torch-tensor front end of the C-ABI (videosys_b200/_lib.py): pointer + shape marshalling only.
 
-Every function enqueues exactly one sm_100a kernel on the current CUDA stream (capturable in a CUDA graph).  CPU tensors are rejected:
+Every function enqueues exactly one sm_90a kernel on the current CUDA stream (capturable in a CUDA graph).  CPU tensors are rejected:
 there is no fallback path.
 """
 import ctypes as C
@@ -74,7 +74,7 @@ def _p(t):
 def require_cuda(t, what: str = "vsb200", half_only: bool = False):
     """The model front ends call this first: there is no CPU execution path (and the kernels take 16-bit activations)."""
     if not t.is_cuda:
-        raise RuntimeError(f"videosys_b200 {what} runs on sm_100a CUDA devices only (no CPU path)")
+        raise RuntimeError(f"videosys_b200 {what} runs on sm_90a CUDA devices only (no CPU path)")
     if half_only and t.dtype not in (torch.bfloat16, torch.float16):
         raise RuntimeError(f"videosys_b200 {what} runs in fp16 / bf16 only")
 
@@ -262,21 +262,15 @@ def gemm_bias_act(a, w, bias=None, act: int = 0, out=None):
 
 
 def gemm_bias_residual(a, w, bias, resid, mod=None, x_mask_u8=None, gate_row: int = -1, B=1, T=1, S=1, out=None):
-    """out = resid + [gate *] (a @ w^T + bias) with the branch fused into the GEMM epilogue.
-    Returns None (nothing launched) when the fused kernel does not take the shape: use the unfused pair then."""
+    """out = resid + [gate *] (a @ w^T + bias) with the branch fused into the GEMM epilogue (out defaults to resid)."""
     lib, st = _prep(a, w, bias, resid, mod, x_mask_u8, out)
     K = a.shape[-1]
     M = a.numel() // K
     N = w.shape[0]
     out = resid if out is None else out
-    with _Timed("gemm", 2 * M * N * K) as tm:
-        rc = _fn(lib, "vsb_gemm_bias_residual", a)(_p(a), _p(w), _p(bias), _p(resid), _p(out), _p(mod), _p(x_mask_u8), gate_row, M,
-                                        N, K, B, T, S, st)
-        if rc == 1:
-            tm.cancel()
-    if rc == 1:
-        return None
-    _lib.check(rc, "gemm_bias_residual")
+    with _Timed("gemm", 2 * M * N * K):
+        _lib.check(_fn(lib, "vsb_gemm_bias_residual", a)(_p(a), _p(w), _p(bias), _p(resid), _p(out), _p(mod), _p(x_mask_u8),
+                                                       gate_row, M, N, K, B, T, S, st), "gemm_bias_residual")
     return out
 
 

@@ -1,4 +1,4 @@
-"""CogVideoX transformer blocks on the vsb200 sm_100a kernels (block level: SURVEY.md section 8 row a15).
+"""CogVideoX transformer blocks on the vsb200 sm_90a kernels (block level: SURVEY.md section 8 row a15).
 
 ``CogVideoXBlockStack`` keeps the reference's state_dict names for ``transformer_blocks.{i}`` (norm1/norm2 =
 CogVideoXLayerNormZero: linear + norm; attn1 = diffusers Attention: to_q|to_k|to_v|norm_q|norm_k|to_out.0;

@@ -1,4 +1,4 @@
-"""Latte transformer blocks on the vsb200 sm_100a kernels (block level: SURVEY.md section 8 row a16).
+"""Latte transformer blocks on the vsb200 sm_90a kernels (block level: SURVEY.md section 8 row a16).
 
 ``LatteBlockStack`` holds the parameters of LatteT2V's ``transformer_blocks`` / ``temporal_transformer_blocks`` under
 the reference's state_dict names (diffusers ``Attention``: attn1/attn2.to_q|to_k|to_v|to_out.0, ``FeedForward``:

@@ -1,4 +1,4 @@
-"""Open-Sora-Plan v1.1.0 transformer (the reference's second ``LatteT2V``) on the vsb200 sm_100a kernels (SURVEY.md section 8
+"""Open-Sora-Plan v1.1.0 transformer (the reference's second ``LatteT2V``) on the vsb200 sm_90a kernels (SURVEY.md section 8
 row (f)4).
 
 Reference: models/transformers/open_sora_plan_v110_transformer_3d.py -- model :2123-2790, spatial block

@@ -1,4 +1,4 @@
-"""Open-Sora-Plan v1.2.0 transformer (``OpenSoraT2V``) on the vsb200 sm_100a kernels (SURVEY.md section 8 row (f)4).
+"""Open-Sora-Plan v1.2.0 transformer (``OpenSoraT2V``) on the vsb200 sm_90a kernels (SURVEY.md section 8 row (f)4).
 
 Reference: models/transformers/open_sora_plan_v120_transformer_3d.py -- model :1464-2112, ``BasicTransformerBlock`` :1092-1455,
 ``Attention`` + ``AttnProcessor2_0`` :647-960, ``RoPE3D`` / ``PositionGetter3D`` :39-118, ``PatchEmbed2D`` :245-369.  One stack
@@ -7,10 +7,9 @@ every head per axis, half-rotation inside each third) -> gate + residual -> text
 key counts) + residual -> modulate -> tanh-GELU feed-forward -> gate + residual; PAB has the spatial and the cross gate and
 caches the UN-gated attention output (:1352-1375, :1391-1416).
 
-Kernels: every Linear = tcgen05 GEMM (q|k|v fused), ``vsb_ln_modulate`` (hidden 2304 = its 9-vector instantiation),
+Kernels: every Linear = wgmma GEMM (q|k|v fused), ``vsb_ln_modulate`` (hidden 2304 = its 9-vector instantiation),
 ``vsb_gate_residual`` / ``vsb_residual_add``, ``vsb_qk_rope_halves`` (half = head_dim / 6, one table row per token) and
-``vsb_attn_flash``, which for head_dim 96 runs the warp-level ``attn_mma`` kernel (csrc/attn_mma.cu: the tcgen05 attention
-kernels are laid out for head_dim 64 / 72).  Sequence parallelism as the reference (:907-916, :937-940, :1861-1866): the
+``vsb_attn_flash`` (csrc/attn_mma.cu, instantiated for head_dim 96).  Sequence parallelism as the reference (:907-916, :937-940, :1861-1866): the
 tokens are split, self-attention exchanges tokens for heads (``comm.ulysses_*``), cross attention stays local.
 
 State-dict compatible with the reference / HF ``LanguageBind/Open-Sora-Plan-v1.2.0`` transformers without a down-sampler

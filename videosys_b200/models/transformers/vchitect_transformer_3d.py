@@ -1,4 +1,4 @@
-"""Vchitect-2.0 (VchitectXLTransformerModel) on the vsb200 sm_100a kernels (SURVEY.md section 8 row (f)4).
+"""Vchitect-2.0 (VchitectXLTransformerModel) on the vsb200 sm_90a kernels (SURVEY.md section 8 row (f)4).
 
 Reference: models/transformers/vchitect_transformer_3d.py (JointTransformerBlock :50-178, model :237-601) and
 models/modules/attentions.py (VchitectAttention :321-638, VchitectAttnProcessor :641-949).  Same module names and
@@ -12,11 +12,11 @@ and three attentions over the concatenated ``[video | text]`` tokens of a frame 
     (complex multiply on interleaved pairs = the pairing of ``vsb_attn_short`` / ``vsb_qk_rmsnorm_rope``), SDPA rounding,
     no q/k norm: ``vsb_attn_short`` (flags 3; its 64-token instantiation carries the reference's 40-frame example) on the
     token-major tensor, or the RoPE pre-pass + ``vsb_attn_flash`` on strided views beyond 64 frames;
-  * cross (:770-803): every token of every frame against the text keys / values of FRAME 0: ``vsb_attn_flash`` (the
-    K/V-resident schedule for <= 320 keys);
+  * cross (:770-803): every token of every frame against the text keys / values of FRAME 0: ``vsb_attn_flash``
+    (per-batch key counts);
   * spatial (:663-705): per frame over its S + L tokens: ``vsb_attn_flash``, head_dim 64.
 
-Every Linear is a tcgen05 GEMM (q|k|v projections of a kind fused into one launch), AdaLayerNormZero /
+Every Linear is a wgmma GEMM (q|k|v projections of a kind fused into one launch), AdaLayerNormZero /
 AdaLayerNormContinuous / norm2 are ``vsb_ln_modulate``, gate + residual is ``vsb_gate_residual``.  What stays torch: the
 ``[video | text]`` concatenations (strided copies), ``attn * 1.1 + cross`` (:897), the 2-D patch convolution and the
 two conditioning MLPs on M = 1 rows.  PAB (temporal, cross, spatial gates in the reference's call order :838-895) caches

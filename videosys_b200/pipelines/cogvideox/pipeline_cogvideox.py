@@ -1,5 +1,5 @@
 """CogVideoX pipeline surface (mirror of videosys/pipelines/cogvideox/pipeline_cogvideox.py: CogVideoXPABConfig :33-44,
-CogVideoXConfig :47-112, CogVideoXPipeline.generate :489-737) around the B200 CogVideoXTransformer3DModel.
+CogVideoXConfig :47-112, CogVideoXPipeline.generate :489-737) around the native CogVideoXTransformer3DModel.
 
 In scope: the config classes, ``generate()``'s signature and shape rules, the CFG + DDIM denoising loop (:692-733) and
 the denoiser.  Out of scope as for OpenSora (SURVEY.md 2.1): T5 encoder, VAE decode (once per video) -- pass
@@ -35,7 +35,7 @@ class CogVideoXConfig:
         self.vae_tiling = vae_tiling
         self.enable_pab = enable_pab
         self.pab_config = pab_config if pab_config is not None else CogVideoXPABConfig()
-        # B200 build extras (as OpenSoraConfig): architecture / weights / out-of-scope stages supplied by the caller
+        # native build extras (as OpenSoraConfig): architecture / weights / out-of-scope stages supplied by the caller
         self.transformer_config = transformer_config
         self.state_dict = state_dict
         self.text_encoder_fn = text_encoder_fn
@@ -48,7 +48,7 @@ class CogVideoXPipeline(ParallelPipelineMixin):
 
     def __init__(self, config: CogVideoXConfig, device=None, dtype: torch.dtype = torch.bfloat16):
         if not torch.cuda.is_available():
-            raise RuntimeError("videosys_b200 pipelines need an sm_100a GPU (no CPU path)")
+            raise RuntimeError("videosys_b200 pipelines need an sm_90a GPU (no CPU path)")
         self._config = config
         self._device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         if config.model_path == "THUDM/CogVideoX-2b":

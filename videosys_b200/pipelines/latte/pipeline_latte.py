@@ -1,5 +1,5 @@
 """Latte pipeline surface (mirror of videosys/pipelines/latte/pipeline_latte.py: LattePABConfig :35-76, LatteConfig
-:127-160, LattePipeline.generate :675-905) around the B200 LatteT2V.
+:127-160, LattePipeline.generate :675-905) around the native LatteT2V.
 
 In scope: the config classes, ``generate()``'s signature, the CFG + DDIM loop (:815-873, learned-sigma split :864-868)
 and the denoiser.  Out of scope as for the other pipelines (SURVEY.md 2.1): T5 encoder, caption cleaning, VAE decode --
@@ -47,7 +47,7 @@ class LatteConfig:
         self.beta_start, self.beta_end, self.beta_schedule, self.variance_type = beta_start, beta_end, beta_schedule, variance_type
         self.enable_pab = enable_pab
         self.pab_config = pab_config if pab_config is not None else LattePABConfig()
-        # B200 build extras: architecture / weights / out-of-scope stages supplied by the caller
+        # native build extras: architecture / weights / out-of-scope stages supplied by the caller
         self.transformer_config = transformer_config
         self.state_dict = state_dict
         self.text_encoder_fn = text_encoder_fn
@@ -59,7 +59,7 @@ class LattePipeline(ParallelPipelineMixin):
 
     def __init__(self, config: LatteConfig, device=None, dtype: torch.dtype = torch.float16):
         if not torch.cuda.is_available():
-            raise RuntimeError("videosys_b200 pipelines need an sm_100a GPU (no CPU path)")
+            raise RuntimeError("videosys_b200 pipelines need an sm_90a GPU (no CPU path)")
         self._config = config
         self._device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         self._dtype = dtype

@@ -1,5 +1,5 @@
 """OpenSora pipeline surface (mirror of videosys/pipelines/open_sora/pipeline_open_sora.py: OpenSoraPABConfig :32-69,
-OpenSoraConfig :126-163, OpenSoraPipeline.generate :426-656) around the B200 STDiT3.
+OpenSoraConfig :126-163, OpenSoraPipeline.generate :426-656) around the native STDiT3.
 
 In scope: the config classes, ``generate()``'s signature, the shape tables, the RFLOW loop and the denoiser.
 Out of scope (SURVEY.md 2.1 rows 7, 9): the T5 text encoder, prompt cleaning and the VAE decode -- they run once per
@@ -83,7 +83,7 @@ class OpenSoraConfig:
         self.enable_flash_attn = enable_flash_attn
         self.enable_pab = enable_pab
         self.pab_config = pab_config if pab_config is not None else OpenSoraPABConfig()
-        # B200 build extras: architecture / weights / out-of-scope stages supplied by the caller
+        # native build extras: architecture / weights / out-of-scope stages supplied by the caller
         self.transformer_config = transformer_config
         self.state_dict = state_dict
         self.text_encoder_fn = text_encoder_fn
@@ -98,7 +98,7 @@ class VideoSysPipelineOutput:
 class OpenSoraPipeline:
     def __init__(self, config: OpenSoraConfig, device=None):
         if not torch.cuda.is_available():
-            raise RuntimeError("videosys_b200 pipelines need an sm_100a GPU (no CPU path)")
+            raise RuntimeError("videosys_b200 pipelines need an sm_90a GPU (no CPU path)")
         self._config = config
         self._device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         import os

@@ -1,12 +1,12 @@
 """Open-Sora-Plan pipeline surface (mirror of videosys/pipelines/open_sora_plan/pipeline_open_sora_plan.py:
 OpenSoraPlanV110PABConfig :41-100, OpenSoraPlanV120PABConfig :103-120, OpenSoraPlanConfig :123-226,
-OpenSoraPlanPipeline.generate :962-1180) around the B200 transformer.
+OpenSoraPlanPipeline.generate :962-1180) around the native transformer.
 
 Version v110 (``LatteT2V``, 65 or 221 frames at 512 x 512, head_dim 72): CFG batch of 2, PNDM steps (incl. its Runge-Kutta
 warm-up: the transformer is evaluated at every entry of ``scheduler.timesteps``), learned-sigma split, PAB with the MLP skip.
 Version v120 (``OpenSoraT2V``, 29 or 93 frames at 480p / 720p, head_dim 96, 3-D RoPE): ancestral Euler steps (the latent is
 scaled by the scheduler before every forward, :1097), PAB with the spatial and the cross gate; its attention runs on the
-warp-level kernel of csrc/attn_mma.cu (the tcgen05 flash kernels are laid out for head_dim 64 / 72: DESIGN.md).  Out of scope as for the other pipelines (SURVEY.md 2.1): T5 encoder and the
+warp-level kernel of csrc/attn_mma.cu (head_dim 64 / 72 run on csrc/attn_wgmma.cu).  Out of scope as for the other pipelines (SURVEY.md 2.1): T5 encoder and the
 causal VAE -- pass ``prompt_embeds`` (+ masks) or a ``text_encoder_fn``; without a ``vae_decode_fn`` the LATENTS are returned.
 dtype fp16 as the reference (:262).
 """
@@ -69,7 +69,7 @@ class OpenSoraPlanConfig:
         if enable_pab and pab_config is None:
             pab_config = OpenSoraPlanV110PABConfig() if version == "v110" else OpenSoraPlanV120PABConfig()
         self.pab_config = pab_config
-        # B200 build extras: architecture / weights / out-of-scope stages supplied by the caller
+        # native build extras: architecture / weights / out-of-scope stages supplied by the caller
         self.transformer_config, self.state_dict = transformer_config, state_dict
         self.text_encoder_fn, self.vae_decode_fn = text_encoder_fn, vae_decode_fn
 
@@ -79,7 +79,7 @@ class OpenSoraPlanPipeline(ParallelPipelineMixin):
 
     def __init__(self, config: OpenSoraPlanConfig, device=None, dtype: torch.dtype = torch.float16):
         if not torch.cuda.is_available():
-            raise RuntimeError("videosys_b200 pipelines need an sm_100a GPU (no CPU path)")
+            raise RuntimeError("videosys_b200 pipelines need an sm_90a GPU (no CPU path)")
         import os
 
         self._config, self._dtype = config, dtype

@@ -1,5 +1,5 @@
 """Vchitect-2.0 pipeline surface (mirror of videosys/pipelines/vchitect/pipeline_vchitect.py: VchitectPABConfig :30-53,
-VchitectConfig :56-127, VchitectXLPipeline.generate :712-1009) around the B200 VchitectXLTransformerModel.
+VchitectConfig :56-127, VchitectXLPipeline.generate :712-1009) around the native VchitectXLTransformerModel.
 
 In scope: the config classes, ``generate()``'s signature, the denoising loop as the reference runs it (:916-954: the
 unconditional and the text branch are two batch-1 forwards, the guidance scale follows the cosine ramp of :943-945,
@@ -41,7 +41,7 @@ class VchitectConfig:
         self.cpu_offload = cpu_offload
         self.enable_pab = enable_pab
         self.pab_config = pab_config if pab_config is not None else VchitectPABConfig()
-        # B200 build extras: architecture / weights / scheduler shift (the HF scheduler_config.json is not in the tree) /
+        # native build extras: architecture / weights / scheduler shift (the HF scheduler_config.json is not in the tree) /
         # out-of-scope stages supplied by the caller
         self.transformer_config = transformer_config
         self.state_dict = state_dict
@@ -55,7 +55,7 @@ class VchitectXLPipeline(ParallelPipelineMixin):
 
     def __init__(self, config: VchitectConfig, device=None, dtype: torch.dtype = torch.bfloat16):
         if not torch.cuda.is_available():
-            raise RuntimeError("videosys_b200 pipelines need an sm_100a GPU (no CPU path)")
+            raise RuntimeError("videosys_b200 pipelines need an sm_90a GPU (no CPU path)")
         import os
 
         self._config = config

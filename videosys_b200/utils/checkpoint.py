@@ -1,4 +1,4 @@
-"""Local checkpoint loading for the B200 denoisers (SURVEY.md section 8(f)3).
+"""Local checkpoint loading for the native denoisers (SURVEY.md section 8(f)3).
 
 The reference pulls weights from the Hugging Face hub (``STDiT3.from_pretrained("hpcai-tech/OpenSora-STDiT-v3")``,
 pipelines/open_sora/pipeline_open_sora.py:222-224; ``CogVideoXTransformer3DModel.from_pretrained(path,
