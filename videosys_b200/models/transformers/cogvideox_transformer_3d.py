@@ -17,15 +17,15 @@ twins) or bf16 (the 5B model's dtype).  ``CogVideoXTransformer3DModel`` below ad
 (reference :315-589; the diffusers pieces -- Timesteps, TimestepEmbedding, get_3d_sincos_pos_embed, AdaLayerNorm --
 restated from their published semantics, diffusers==0.30.0: parity unpinned for those, SURVEY.md 8c).
 """
-import math
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
 from ... import kernels
 from ...core.distributed import comm
-from ...core.distributed.parallel_mgr import ParallelManager
 from ...core.pab import pab_mgr
+from ._attention import apply_rope_, packed_self_attention, ulysses_attention
+from ._common import fused_linear, parallel_manager, pos_embed_2d, sincos_1d, timestep_sinusoid
 
 
 class _LayerNormZero(nn.Module):
@@ -69,15 +69,7 @@ class CogVideoXBlock(nn.Module):
         self.block_idx = block_idx
         self.attn_count = 0
         self.last_attn = None
-        self._qkv = None
-
-    def fused_qkv(self):
-        a = self.attn1
-        key = tuple((t.data_ptr(), t._version, t.dtype) for t in (a.to_q.weight, a.to_k.weight, a.to_v.weight, a.to_q.bias))
-        if self._qkv is None or self._qkv[0] != key:  # rebuilt after load_state_dict / .to(dtype or device)
-            self._qkv = (key, torch.cat([a.to_q.weight, a.to_k.weight, a.to_v.weight], 0).contiguous(),
-                         torch.cat([a.to_q.bias, a.to_k.bias, a.to_v.bias], 0).contiguous())
-        return self._qkv[1], self._qkv[2]
+        self._fused = {}
 
 
 class CogVideoXBlockStack(nn.Module):
@@ -89,12 +81,6 @@ class CogVideoXBlockStack(nn.Module):
         self.transformer_blocks = nn.ModuleList(
             [CogVideoXBlock(dim, num_attention_heads, attention_head_dim, time_embed_dim, i) for i in range(num_layers)]
         )
-
-    def load_state_dict(self, *a, **k):
-        r = super().load_state_dict(*a, **k)
-        for b in self.transformer_blocks:
-            b._qkv = None
-        return r
 
     def reset_pab_state(self):
         for b in self.transformer_blocks:
@@ -143,29 +129,15 @@ class CogVideoXBlockStack(nn.Module):
             if reuse:
                 a = blk.last_attn
             else:
-                w, bias = blk.fused_qkv()
-                qkv = K.gemm_bias_act(ncat.view(B * N, C), w, bias)
                 at = blk.attn1
+                qkv = K.gemm_bias_act(ncat.view(B * N, C), *fused_linear(blk._fused, at.to_q, at.to_k, at.to_v))
                 K.qk_layernorm_(qkv, at.norm_q.weight, at.norm_q.bias, at.norm_k.weight, at.norm_k.bias, H, D, eps=1e-6)
                 if sp_group is None:
                     if rope is not None:
-                        K.qk_rmsnorm_(qkv, None, None, H, D, rope_cos=rope[0], rope_sin=rope[1], pos_div=1, pos_mod=N)
-                    q3 = qkv.view(-1, 3, C)
-                    o = K.attn_flash(q3[:, 0], q3[:, 1], q3[:, 2], B, N, N, H, D, 3 * C, N * 3 * C, 3 * C, N * 3 * C, D**-0.5)
-                else:
-                    full = comm.ulysses_scatter_heads(qkv.view(B, N, 3, H, D), Nt, sp_group)  # every row, H / sp heads
-                    Lf, Hn = full.shape[1], full.shape[3]
-                    Cn, Lv = Hn * D, Nt + n_video
-                    if rope is not None:  # positions of the gathered sequence (the table covers the pad rows with identity)
-                        full = full.contiguous()
-                        K.qk_rmsnorm_(full, None, None, Hn, D, rope_cos=rope[0], rope_sin=rope[1], pos_div=1, pos_mod=Lf)
-                    f3 = full.view(B * Lf, 3, Cn)
-                    of = torch.empty(B, Lf, Cn, dtype=qkv.dtype, device=qkv.device)
-                    if Lf > Lv:
-                        of[:, Lv:].zero_()
-                    K.attn_flash(f3[:, 0], f3[:, 1], f3[:, 2], B, Lv, Lv, Hn, D, 3 * Cn, Lf * 3 * Cn, 3 * Cn, Lf * 3 * Cn,
-                                 D**-0.5, out=of, out_row_stride=Cn, out_batch_stride=Lf * Cn)
-                    o = comm.ulysses_gather_heads(of, Nt, sp_group).contiguous()  # my rows, every head
+                        apply_rope_(qkv, rope, H, D, pos_div=1, pos_mod=N)
+                    o = packed_self_attention(qkv, B, N, H, D, D**-0.5)
+                else:  # every row on H / sp heads; the rope table covers the pad rows with identity
+                    o = ulysses_attention(qkv.view(B, N, 3, H, D), Nt, Nt + n_video, sp_group, D**-0.5, rope=rope)
                 a = K.gemm_bias_act(o, at.to_out[0].weight, at.to_out[0].bias)  # [B, N, C] = [text | video]
                 if pab_on:
                     blk.last_attn = a
@@ -184,13 +156,6 @@ class CogVideoXBlockStack(nn.Module):
 
 
 # ---- the whole denoiser (reference CogVideoXTransformer3DModel :315-589), 2B configuration --------------------------------
-def _sincos_1d(embed_dim: int, pos: torch.Tensor) -> torch.Tensor:
-    """diffusers get_1d_sincos_pos_embed_from_grid: [sin(pos * w) | cos(pos * w)], w = 10000^(-2i/embed_dim), float64."""
-    omega = 1.0 / 10000 ** (torch.arange(embed_dim // 2, dtype=torch.float64) / (embed_dim / 2.0))
-    out = pos.reshape(-1).double()[:, None] * omega[None]
-    return torch.cat([out.sin(), out.cos()], dim=1)
-
-
 def get_3d_sincos_pos_embed(embed_dim, spatial_size, temporal_size, spatial_interpolation_scale=1.0,
                             temporal_interpolation_scale=1.0) -> torch.Tensor:
     """diffusers.models.embeddings.get_3d_sincos_pos_embed (0.30.0), call site reference :412-418: a quarter of the
@@ -198,13 +163,9 @@ def get_3d_sincos_pos_embed(embed_dim, spatial_size, temporal_size, spatial_inte
     assert embed_dim % 4 == 0
     W, H = spatial_size
     d_sp, d_t = 3 * embed_dim // 4, embed_dim // 4
-    gh = torch.arange(H, dtype=torch.float32) / spatial_interpolation_scale
-    gw = torch.arange(W, dtype=torch.float32) / spatial_interpolation_scale
-    grid_w, grid_h = torch.meshgrid(gw, gh, indexing="xy")  # np.meshgrid(grid_w, grid_h): both [H, W]
-    emb_h = _sincos_1d(d_sp // 2, grid_w)  # the library feeds grid[0] (= the w coordinates) to its "emb_h"
-    emb_w = _sincos_1d(d_sp // 2, grid_h)
-    sp = torch.cat([emb_h, emb_w], dim=1)  # [H*W, d_sp]
-    tm = _sincos_1d(d_t, torch.arange(temporal_size, dtype=torch.float32) / temporal_interpolation_scale)  # [T, d_t]
+    s = spatial_interpolation_scale
+    sp = pos_embed_2d(d_sp, (H, W), (H, W), (s, s))  # [H*W, d_sp]
+    tm = sincos_1d(d_t, torch.arange(temporal_size, dtype=torch.float32) / temporal_interpolation_scale)  # [T, d_t]
     out = torch.cat([tm[:, None, :].expand(-1, H * W, -1), sp[None].expand(temporal_size, -1, -1)], dim=-1)
     return out.float()
 
@@ -293,26 +254,11 @@ class CogVideoXTransformer3DModel(nn.Module):
         return build_from_pretrained(cls, path, subfolder, **config_overrides)
 
     def enable_parallel(self, dp_size=None, sp_size=None, enable_cp=None):
-        """Reference :462-474: CFG parallelism takes a factor 2 out of an even sp_size when ``enable_cp``."""
-        dp_size, sp_size = dp_size or 1, sp_size or 1
-        cp_size = 1
-        if enable_cp and sp_size % 2 == 0:
-            sp_size, cp_size = sp_size // 2, 2
-        if self.config.num_attention_heads % sp_size:
-            raise ValueError(f"Number of heads {self.config.num_attention_heads} must be divisible by sequence parallel "
-                             f"size {sp_size}")
-        self.parallel_manager = ParallelManager(dp_size, cp_size, sp_size)
+        """Reference :462-474."""
+        self.parallel_manager = parallel_manager(dp_size, sp_size, enable_cp, self.config.num_attention_heads)
 
     def reset_pab_state(self):
         self._stack[0].reset_pab_state()
-
-    def _time_proj(self, timesteps: torch.Tensor) -> torch.Tensor:
-        """diffusers Timesteps(dim, flip_sin_to_cos, freq_shift): fp32 [cos | sin] (flipped) sinusoid."""
-        half = self.inner_dim // 2
-        exponent = -math.log(10000.0) * torch.arange(half, dtype=torch.float32, device=timesteps.device) / (half - self.freq_shift)
-        emb = timesteps[:, None].float() * exponent.exp()[None]
-        emb = torch.cat([emb.sin(), emb.cos()], dim=-1)
-        return torch.cat([emb[:, half:], emb[:, :half]], dim=-1) if self.flip else emb
 
     @torch.no_grad()
     def forward(self, hidden_states, encoder_hidden_states, timestep, timestep_cond=None, image_rotary_emb=None,
@@ -330,7 +276,7 @@ class CogVideoXTransformer3DModel(nn.Module):
         B, Fr, Cin, H, W = hidden_states.shape
         p, C = self.config.patch_size, self.inner_dim
         te = self.time_embedding
-        t_emb = self._time_proj(timestep).to(dt)
+        t_emb = timestep_sinusoid(timestep, self.inner_dim, self.flip, self.freq_shift).to(dt)
         emb = K.gemm_bias_act(F.silu(K.gemm_bias_act(t_emb, te.linear_1.weight, te.linear_1.bias)), te.linear_2.weight,
                               te.linear_2.bias)  # [B, 512]
         txt = K.gemm_bias_act(encoder_hidden_states.to(dt).contiguous(), self.patch_embed.text_proj.weight,

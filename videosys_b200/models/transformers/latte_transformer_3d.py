@@ -16,17 +16,17 @@ table, Timesteps / TimestepEmbedding inside PixArtAlphaCombinedTimestepSizeEmbed
 restated from their published semantics (diffusers==0.30.0: parity unpinned for those, SURVEY.md 8c).  Compute dtype:
 fp16 (the reference's, pipeline_latte.py:201) or bf16.  PAB: spatial / temporal / cross broadcast and the MLP skip.
 """
-import math
 from typing import Optional
 
 import torch
 import torch.nn as nn
-import torch.nn.functional as F
 
 from ... import kernels
 from ...core.distributed import comm
-from ...core.distributed.parallel_mgr import ParallelManager
 from ...core.pab import pab_mgr
+from ._attention import apply_rope_, cross_attention, packed_self_attention, temporal_attention
+from ._common import (AdaLNSingle, Lin2, PatchEmbed2D, ada_norm_single, ada_norm_single_out, fused_linear, parallel_manager,
+                      patch_embed_frames, pos_embed_2d, sincos_1d)
 
 
 class _Attn(nn.Module):
@@ -68,20 +68,6 @@ class LatteBlock(nn.Module):
         # reference attributes: spatial_count / count (temporal), cross_count, mlp_count; spatial_last / last_out, cross_last
         self.attn_count = self.cross_count = self.mlp_count = 0
         self.last_attn = self.last_cross = None
-
-    def fused(self, which: str):
-        """Concatenated projection weights, rebuilt when the parameters change (load_state_dict / .to)."""
-        a = self.attn1 if which == "qkv" else self.attn2
-        mods = (a.to_q, a.to_k, a.to_v) if which == "qkv" else (a.to_k, a.to_v)
-        key = tuple((m.weight.data_ptr(), m.weight._version, m.weight.dtype) for m in mods)
-        c = self._fused.get(which)
-        if c is None or c[0] != key:
-            c = self._fused[which] = (key, torch.cat([m.weight for m in mods], 0).contiguous(),
-                                      torch.cat([m.bias for m in mods], 0).contiguous())
-        return c[1], c[2]
-
-    def invalidate(self):
-        self._fused = {}
 
 
 class LatteBlockStack(nn.Module):
@@ -141,29 +127,15 @@ class LatteBlockStack(nn.Module):
                                                       gather_pad=comm.get_pad("temporal")).contiguous()
                         Ft, St = xm.shape[1], xm.shape[2]
                         xm = xm.view(B * Ft * St, C)
-                    wqkv, bqkv = blk.fused("qkv")
-                    qkv = K.gemm_bias_act(xm, wqkv, bqkv)
-                    if rope is not None:
-                        rc, rs, half = rope["temporal" if blk.temporal else "spatial"]
-                        if blk.temporal:
-                            K.qk_rope_halves_(qkv, rc, rs, H, D, half, pos_div=St, pos_mod=Ft)
-                        else:
-                            K.qk_rope_halves_(qkv, rc, rs, H, D, half, pos_div=1, pos_mod=S)
+                    a1 = blk.attn1
+                    qkv = K.gemm_bias_act(xm, *fused_linear(blk._fused, a1.to_q, a1.to_k, a1.to_v))
                     if blk.temporal:
-                        if Ft <= 32:
-                            o = K.attn_short(qkv.view(-1, 3, H, D), None, None, None, None, B, St, Ft * St, 1, St, Ft, H, D, D**-0.5, flags=3)
-                        else:  # long videos: the flash kernel over strided views (batch = patch, row = frame)
-                            o = torch.empty(B * Ft * St, C, dtype=x.dtype, device=x.device)
-                            q3 = qkv.view(B, Ft * St, 3, C)
-                            for b in range(B):
-                                K.attn_flash(q3[b, :, 0], q3[b, :, 1], q3[b, :, 2], St, Ft, Ft, H, D, St * 3 * C, 3 * C, St * 3 * C, 3 * C,
-                                             D**-0.5, out=o[b * Ft * St:], out_row_stride=St * C, out_batch_stride=C)
+                        o = temporal_attention(qkv, B, Ft, St, H, D, D**-0.5, 32, sdpa=True,
+                                               rope=None if rope is None else rope["temporal"])
                     else:
-                        q3 = qkv.view(-1, 3, C)
-                        if S >= 30:
-                            o = K.attn_flash(q3[:, 0], q3[:, 1], q3[:, 2], B * Fr, S, S, H, D, 3 * C, S * 3 * C, 3 * C, S * 3 * C, D**-0.5)
-                        else:
-                            o = K.attn_short(qkv.view(-1, 3, H, D), None, None, None, None, B * Fr, 1, S, 0, 1, S, H, D, D**-0.5, flags=3)
+                        if rope is not None:
+                            apply_rope_(qkv, rope["spatial"], H, D, pos_div=1, pos_mod=S)
+                        o = packed_self_attention(qkv, B * Fr, S, H, D, D**-0.5, short_max=29, sdpa=True)
                     y = K.gemm_bias_act(o.view(-1, C), blk.attn1.to_out[0].weight, blk.attn1.to_out[0].bias)
                     if switch:  # patch shard -> frame shard (scatter F, gather S)
                         y = comm.all_to_all_with_pad(y.view(B, Ft, St, C), sp_group, scatter_dim=1, gather_dim=2,
@@ -185,10 +157,8 @@ class LatteBlockStack(nn.Module):
                     else:
                         a2 = blk.attn2
                         q = K.gemm_bias_act(xf, a2.to_q.weight, a2.to_q.bias)
-                        wkv, bkv = blk.fused("kv")
-                        kv = K.gemm_bias_act(enc2, wkv, bkv).view(-1, 2, C)
-                        o = K.attn_flash(q, kv[:, 0], kv[:, 1], B, Fr * S, L, H, D, C, Fr * S * C, 2 * C, L * 2 * C, D**-0.5,
-                                         kv_lens=enc_lens)
+                        kv = K.gemm_bias_act(enc2, *fused_linear(blk._fused, a2.to_k, a2.to_v)).view(-1, 2, C)
+                        o = cross_attention(q, kv, B, Fr * S, L, H, D, D**-0.5, kv_lens=enc_lens)
                         out = blk.last_cross if (pab_on and blk.last_cross is not None and blk.last_cross.shape == xf.shape) else None
                         xc = K.gemm_bias_act(o, a2.to_out[0].weight, a2.to_out[0].bias, out=out)
                         if pab_on:
@@ -216,53 +186,6 @@ class LatteBlockStack(nn.Module):
 
 
 # ---- the whole denoiser (reference LatteT2V :846-1470, ada_norm_single / PixArt-alpha conditioning) ------------------------
-def _sincos_1d(embed_dim: int, pos: torch.Tensor) -> torch.Tensor:
-    """diffusers get_1d_sincos_pos_embed_from_grid: [sin | cos], float64 omega."""
-    omega = 1.0 / 10000 ** (torch.arange(embed_dim // 2, dtype=torch.float64) / (embed_dim / 2.0))
-    out = pos.reshape(-1).double()[:, None] * omega[None]
-    return torch.cat([out.sin(), out.cos()], dim=1)
-
-
-def get_2d_sincos_pos_embed(embed_dim: int, grid_size: int, base_size: int = 16, interpolation_scale: float = 1.0) -> torch.Tensor:
-    """diffusers.models.embeddings.get_2d_sincos_pos_embed (0.30.0) as PatchEmbed uses it: [grid*grid, D] float32."""
-    g = torch.arange(grid_size, dtype=torch.float32) / (grid_size / base_size) / interpolation_scale
-    grid_w, grid_h = torch.meshgrid(g, g, indexing="xy")  # np.meshgrid(grid_w, grid_h): w first
-    return torch.cat([_sincos_1d(embed_dim // 2, grid_w), _sincos_1d(embed_dim // 2, grid_h)], dim=1).float()
-
-
-class _TimestepEmbedder(nn.Module):
-    def __init__(self, cin, cout):
-        super().__init__()
-        self.linear_1 = nn.Linear(cin, cout)
-        self.linear_2 = nn.Linear(cout, cout)
-
-
-class _CombinedEmb(nn.Module):
-    def __init__(self, dim):
-        super().__init__()
-        self.timestep_embedder = _TimestepEmbedder(256, dim)
-
-
-class _AdaLNSingle(nn.Module):
-    def __init__(self, dim):
-        super().__init__()
-        self.emb = _CombinedEmb(dim)
-        self.linear = nn.Linear(dim, 6 * dim)
-
-
-class _CaptionProjection(nn.Module):
-    def __init__(self, cin, dim):
-        super().__init__()
-        self.linear_1 = nn.Linear(cin, dim)
-        self.linear_2 = nn.Linear(dim, dim)
-
-
-class _PatchEmbed2D(nn.Module):
-    def __init__(self, patch, cin, dim):
-        super().__init__()
-        self.proj = nn.Conv2d(cin, dim, kernel_size=(patch, patch), stride=patch, bias=True)
-
-
 class LatteT2V(nn.Module):
     """State-dict compatible with the reference / HF ``maxin-cn/Latte-1`` transformer (same parameter names), forward on the
     vsb200 kernels.  ``enable_parallel`` as the reference (:1127-1139): frame-sharded DSP (temporal blocks switch to a
@@ -283,19 +206,18 @@ class LatteT2V(nn.Module):
                                            num_attention_heads=num_attention_heads, attention_head_dim=attention_head_dim,
                                            num_layers=num_layers))()
         self.inner_dim, self.patch_size, self.out_channels, self.eps = dim, patch_size, out_channels, norm_eps
-        self.pos_embed = _PatchEmbed2D(patch_size, in_channels, dim)
+        self.pos_embed = PatchEmbed2D(patch_size, in_channels, dim)
         grid = sample_size // patch_size
-        self.register_buffer("pos_table", get_2d_sincos_pos_embed(dim, grid, base_size=grid,
-                                                                  interpolation_scale=max(sample_size // 64, 1))[None], persistent=False)
-        self.adaln_single = _AdaLNSingle(dim)
-        self.caption_projection = _CaptionProjection(caption_channels, dim)
+        self.register_buffer("pos_table", self._pos_2d(grid, grid)[None], persistent=False)
+        self.adaln_single = AdaLNSingle(dim)
+        self.caption_projection = Lin2(caption_channels, dim)
         stack = LatteBlockStack(dim, num_attention_heads, num_layers)
         self.transformer_blocks = stack.transformer_blocks
         self.temporal_transformer_blocks = stack.temporal_transformer_blocks
         self._stack = [stack]
         self.scale_shift_table = nn.Parameter(torch.randn(2, dim) / dim**0.5)
         self.proj_out = nn.Linear(dim, patch_size * patch_size * out_channels)
-        self.register_buffer("temp_pos_embed", _sincos_1d(dim, torch.arange(video_length).float()).float()[None], persistent=False)
+        self.register_buffer("temp_pos_embed", sincos_1d(dim, torch.arange(video_length).float()).float()[None], persistent=False)
         self.parallel_manager = None
 
     @classmethod
@@ -306,23 +228,17 @@ class LatteT2V(nn.Module):
         return build_from_pretrained(cls, path, subfolder, **config_overrides)
 
     def enable_parallel(self, dp_size=None, sp_size=None, enable_cp=None):
-        """Reference :1127-1139: CFG parallelism takes a factor 2 out of an even sp_size when ``enable_cp``."""
-        dp_size, sp_size = dp_size or 1, sp_size or 1
-        cp_size = 1
-        if enable_cp and sp_size % 2 == 0:
-            sp_size, cp_size = sp_size // 2, 2
-        self.parallel_manager = ParallelManager(dp_size, cp_size, sp_size)
+        """Reference :1127-1139."""
+        self.parallel_manager = parallel_manager(dp_size, sp_size, enable_cp)
 
     def reset_pab_state(self):
         self._stack[0].reset_pab_state()
 
-    @staticmethod
-    def _time_proj(timesteps: torch.Tensor, dim: int = 256) -> torch.Tensor:
-        """diffusers Timesteps(256, flip_sin_to_cos=True, downscale_freq_shift=0): fp32 [cos | sin]."""
-        half = dim // 2
-        exponent = -math.log(10000.0) * torch.arange(half, dtype=torch.float32, device=timesteps.device) / half
-        emb = timesteps[:, None].float() * exponent.exp()[None]
-        return torch.cat([emb.cos(), emb.sin()], dim=-1)
+    def _pos_2d(self, h, w):
+        """diffusers PatchEmbed's 2-D sin-cos table for an h x w patch grid (square: h == w)."""
+        base = self.config.sample_size // self.patch_size
+        s = max(self.config.sample_size // 64, 1)
+        return pos_embed_2d(self.inner_dim, (h, w), (base, base), (s, s))
 
     @torch.no_grad()
     def forward(self, hidden_states, timestep=None, all_timesteps=None, encoder_hidden_states=None, added_cond_kwargs=None,
@@ -341,27 +257,13 @@ class LatteT2V(nn.Module):
         if cpar:  # reference :1198-1216: the CFG pair is split across the cp group
             hidden_states, timestep, encoder_hidden_states = (
                 comm.split_sequence(v, pm.cp_group, dim=0) for v in (hidden_states, timestep, encoder_hidden_states))
-        B, Cin, Fr, H, W = hidden_states.shape
+        B, _, Fr, H, W = hidden_states.shape
         p, C = self.patch_size, self.inner_dim
         h, w = H // p, W // p
         S = h * w
-        pos = self.pos_table if S == self.pos_table.shape[1] else get_2d_sincos_pos_embed(
-            C, h, base_size=self.config.sample_size // p, interpolation_scale=max(self.config.sample_size // 64, 1))[None].to(hidden_states.device)
-        # PatchEmbed (:1245): 2 x 2 conv per frame + 2-D sincos table; one kernel on the [B, C, F, H, W] latent as it is
-        x = K.patch_embed(hidden_states.to(dt).contiguous(), self.pos_embed.proj.weight, self.pos_embed.proj.bias,
-                          pos[0].to(dt).contiguous(), p, p)
-        if x is None:  # not a 16-tap embedding: the eager chain (cuDNN conv, once per step)
-            x = hidden_states.to(dt).permute(0, 2, 1, 3, 4).reshape(B * Fr, Cin, H, W)
-            x = self.pos_embed.proj(x).flatten(2).transpose(1, 2)
-            x = (x + pos.to(dt)).reshape(B, Fr, S, C)
-        te = self.adaln_single.emb.timestep_embedder
-        t_emb = self._time_proj(timestep).to(dt)
-        embedded = K.gemm_bias_act(F.silu(K.gemm_bias_act(t_emb, te.linear_1.weight, te.linear_1.bias)), te.linear_2.weight,
-                                   te.linear_2.bias)  # [B, C]
-        t6 = K.gemm_bias_act(F.silu(embedded), self.adaln_single.linear.weight, self.adaln_single.linear.bias)  # [B, 6C]
-        cp = self.caption_projection
-        enc = K.gemm_bias_act(K.gemm_bias_act(encoder_hidden_states.to(dt).contiguous(), cp.linear_1.weight, cp.linear_1.bias, act=1),
-                              cp.linear_2.weight, cp.linear_2.bias)  # [B, L, C]
+        pos = self.pos_table if S == self.pos_table.shape[1] else self._pos_2d(h, h)[None].to(hidden_states.device)
+        x = patch_embed_frames(self.pos_embed, hidden_states, pos, p, dt)  # PatchEmbed (:1245)
+        embedded, t6, enc = ada_norm_single(self.adaln_single, self.caption_projection, timestep, encoder_hidden_states, dt)
         if pab_mgr.enable_pab() and ts_int is None:
             ts_int = int(timestep[0])
         if all_timesteps is not None and torch.is_tensor(all_timesteps):
@@ -376,10 +278,8 @@ class LatteT2V(nn.Module):
                 tpe = comm.split_sequence(tpe, pm.sp_group, dim=1, pad=comm.get_pad("temporal"))
             Fr = x.shape[1]
         x = self._stack[0](x, enc, t6, tpe, ts_int=ts_int, all_timesteps=all_timesteps, sp_group=pm.sp_group if sp else None)
-        # output head (:1436-1443): LayerNorm (no affine) -> * (1 + scale) + shift with table + embedded timestep -> proj_out
-        tab6 = torch.cat([self.scale_shift_table, self.scale_shift_table.new_zeros(4, C)], 0)
-        mod = K.modulation_table(tab6, torch.cat([embedded, embedded, embedded.new_zeros(B, 4 * C)], 1).contiguous(), None)
-        y = K.ln_modulate(x.view(B, Fr * S, C), mod, None, 0, 1, B, Fr, S, eps=self.eps)
+        # output head (:1436-1443)
+        y = ada_norm_single_out(self.scale_shift_table, embedded, x.view(B, Fr * S, C), B, Fr, S, self.eps)
         y = K.gemm_bias_act(y, self.proj_out.weight, self.proj_out.bias)  # [B, F*S, p*p*Cout]
         if sp:  # the head is row-wise: run on the local frames, gather its 36x narrower output (reference gathers first, :1428-1429)
             y = comm.gather_sequence(y.view(B, Fr, S, -1), pm.sp_group, dim=1, pad=comm.get_pad("temporal"))

@@ -19,36 +19,22 @@ compression (``compress_kv_factor`` > 1, :1190-1208), joint image training (``us
 attention masks (the pipeline passes all-ones, pipeline_open_sora_plan.py:1119).  The diffusers leaf classes the
 reference file imports (GELU, Timesteps, TimestepEmbedding) are restated from their published semantics.
 """
-import math
-
 import torch
 import torch.nn as nn
-import torch.nn.functional as F
 
 from ... import kernels
 from ...core.distributed import comm
-from ...core.distributed.parallel_mgr import ParallelManager
 from ...core.pab import pab_mgr
-from .latte_transformer_3d import LatteBlockStack, _AdaLNSingle, _PatchEmbed2D, _sincos_1d
+from ._common import (AdaLNSingle, Lin2, PatchEmbed2D, ada_norm_single, ada_norm_single_out, parallel_manager,
+                      patch_embed_frames, pos_embed_2d, sincos_1d, text_lens)
+from .latte_transformer_3d import LatteBlockStack
 
 
-def get_2d_sincos_pos_embed(embed_dim, grid_hw, base_size, interpolation_scale=1.0):
-    """reference :75-106: [h*w, D] float32; first half of the channels from the w coordinate (np.meshgrid(grid_w, grid_h)),
-    second half from h; both axes divided by (extent / base_size) and the interpolation scale."""
-    gh, gw = grid_hw
-    ys = torch.arange(gh, dtype=torch.float32) / (gh / base_size) / interpolation_scale
-    xs = torch.arange(gw, dtype=torch.float32) / (gw / base_size) / interpolation_scale
-    grid_w, grid_h = torch.meshgrid(xs, ys, indexing="xy")  # [gh, gw] each
-    return torch.cat([_sincos_1d(embed_dim // 2, grid_w), _sincos_1d(embed_dim // 2, grid_h)], dim=1).float()
-
-
-class _CaptionProjection(nn.Module):
+class _CaptionProjection(Lin2):
     """reference :340-358 (linear_1 -> tanh-GELU -> linear_2; the unused y_embedding buffer is part of the state dict)."""
 
     def __init__(self, cin, dim, num_tokens=120):
-        super().__init__()
-        self.linear_1 = nn.Linear(cin, dim)
-        self.linear_2 = nn.Linear(dim, dim)
+        super().__init__(cin, dim)
         self.register_buffer("y_embedding", torch.randn(num_tokens, cin) / cin**0.5)
 
 
@@ -98,12 +84,12 @@ class LatteT2V(nn.Module):
         if interpolation_scale_1d is None:  # :2240-2247
             interpolation_scale_1d = (video_length - 1) // 16 if video_length % 2 == 1 else video_length // 16
         self.scale_1d = max(interpolation_scale_1d, 1)
-        self.pos_embed = _PatchEmbed2D(patch_size, in_channels, dim)
+        self.pos_embed = PatchEmbed2D(patch_size, in_channels, dim)
         gh, gw = sample_size[0] // patch_size, sample_size[1] // patch_size
         g = int((gh * gw) ** 0.5)  # reference PatchEmbed :387-389: a square table of int(sqrt(num_patches))
-        self.register_buffer("pos_table", get_2d_sincos_pos_embed(dim, (g, g), gh, self.scale_2d)[None], persistent=False)
         self._grid = (gh, gw)
-        self.adaln_single = _AdaLNSingle(dim)
+        self.register_buffer("pos_table", self._pos_2d(g, g)[None], persistent=False)
+        self.adaln_single = AdaLNSingle(dim)
         self.caption_projection = _CaptionProjection(caption_channels, dim)
         stack = LatteBlockStack(dim, num_attention_heads, num_layers)
         self.transformer_blocks = stack.transformer_blocks
@@ -111,7 +97,7 @@ class LatteT2V(nn.Module):
         self._stack = [stack]
         self.scale_shift_table = nn.Parameter(torch.randn(2, dim) / dim**0.5)
         self.proj_out = nn.Linear(dim, patch_size * patch_size * out_channels)
-        tpe = _sincos_1d(dim, torch.arange(0, video_length).unsqueeze(1) / self.scale_1d)  # :109-112
+        tpe = sincos_1d(dim, torch.arange(0, video_length).unsqueeze(1) / self.scale_1d)  # :109-112
         self.register_buffer("temp_pos_embed", tpe.float()[None], persistent=False)
         self._rope = {}
         self.parallel_manager = None
@@ -125,11 +111,7 @@ class LatteT2V(nn.Module):
 
     def enable_parallel(self, dp_size=None, sp_size=None, enable_cp=None):
         """Reference :2344-2356."""
-        dp_size, sp_size = dp_size or 1, sp_size or 1
-        cp_size = 1
-        if enable_cp and sp_size % 2 == 0:
-            sp_size, cp_size = sp_size // 2, 2
-        self.parallel_manager = ParallelManager(dp_size, cp_size, sp_size)
+        self.parallel_manager = parallel_manager(dp_size, sp_size, enable_cp)
 
     def reset_pab_state(self):
         self._stack[0].reset_pab_state()
@@ -143,25 +125,10 @@ class LatteT2V(nn.Module):
                                "temporal": rope_tables(D, [torch.arange(Fr)], self.scale_1d, dtype, device)}
         return self._rope[key]
 
-    @staticmethod
-    def _time_proj(timesteps: torch.Tensor, dim: int = 256) -> torch.Tensor:
-        half = dim // 2
-        exponent = -math.log(10000.0) * torch.arange(half, dtype=torch.float32, device=timesteps.device) / half
-        emb = timesteps[:, None].float() * exponent.exp()[None]
-        return torch.cat([emb.cos(), emb.sin()], dim=-1)
-
-    @staticmethod
-    def _text_lens(mask, B, L):
-        """encoder_attention_mask [B, L] or [B, 1, L] (1 = keep) -> valid key counts; the kernel masks a suffix."""
-        if mask is None:
-            return None
-        m = mask.reshape(B, -1)[:, -L:].to(torch.bool).cpu()
-        lens = m.sum(-1)
-        if not torch.equal(m, torch.arange(L)[None] < lens[:, None]):
-            raise NotImplementedError("videosys_b200: the text mask must keep a prefix of the tokens (tokenizer padding)")
-        if int(lens.min()) == 0:
-            raise NotImplementedError("videosys_b200: a sample with no valid text token")
-        return [int(v) for v in lens]
+    def _pos_2d(self, h, w):
+        """reference get_2d_sincos_pos_embed :75-106: both axes divided by (extent / grid height) and the 2-D scale."""
+        base, s = self._grid[0], self.scale_2d
+        return pos_embed_2d(self.inner_dim, (h, w), (base, base), (s, s))
 
     @torch.no_grad()
     def forward(self, hidden_states, timestep=None, all_timesteps=None, encoder_hidden_states=None, added_cond_kwargs=None,
@@ -186,32 +153,20 @@ class LatteT2V(nn.Module):
                 comm.split_sequence(v, pm.cp_group, dim=0) for v in (hidden_states, timestep, encoder_hidden_states))
             if encoder_attention_mask is not None:
                 encoder_attention_mask = comm.split_sequence(encoder_attention_mask, pm.cp_group, dim=0)
-        B, Cin, Fr, H, W = hidden_states.shape
+        B, _, Fr, H, W = hidden_states.shape
         if Fr != self.video_length:
             raise ValueError(f"{Fr} latent frames, but the temporal position table has {self.video_length} (reference :2656)")
         p, C = self.patch_size, self.inner_dim
         h, w = H // p, W // p
         S = h * w
         L = encoder_hidden_states.shape[1]
-        lens = self._text_lens(encoder_attention_mask, B, L)
+        lens = text_lens(encoder_attention_mask, B, L)
         if (h, w) == self._grid and S == self.pos_table.shape[1]:
             pos = self.pos_table
         else:  # reference PatchEmbed.forward :412-420
-            pos = get_2d_sincos_pos_embed(C, (h, w), self._grid[0], self.scale_2d)[None].to(hidden_states.device)
-        x = K.patch_embed(hidden_states.to(dt).contiguous(), self.pos_embed.proj.weight, self.pos_embed.proj.bias,
-                          pos[0].to(dt).contiguous(), p, p)
-        if x is None:  # not a 16-tap embedding: the eager chain (cuDNN conv, once per step)
-            x = hidden_states.to(dt).permute(0, 2, 1, 3, 4).reshape(B * Fr, Cin, H, W)
-            x = self.pos_embed.proj(x).flatten(2).transpose(1, 2)
-            x = (x + pos.to(dt)).reshape(B, Fr, S, C)
-        te = self.adaln_single.emb.timestep_embedder
-        t_emb = self._time_proj(timestep).to(dt)
-        embedded = K.gemm_bias_act(F.silu(K.gemm_bias_act(t_emb, te.linear_1.weight, te.linear_1.bias)), te.linear_2.weight,
-                                   te.linear_2.bias)  # [B, C]
-        t6 = K.gemm_bias_act(F.silu(embedded), self.adaln_single.linear.weight, self.adaln_single.linear.bias)  # [B, 6C]
-        cp = self.caption_projection
-        enc = K.gemm_bias_act(K.gemm_bias_act(encoder_hidden_states.to(dt).contiguous(), cp.linear_1.weight, cp.linear_1.bias, act=1),
-                              cp.linear_2.weight, cp.linear_2.bias)  # [B, L, C]
+            pos = self._pos_2d(h, w)[None].to(hidden_states.device)
+        x = patch_embed_frames(self.pos_embed, hidden_states, pos, p, dt)
+        embedded, t6, enc = ada_norm_single(self.adaln_single, self.caption_projection, timestep, encoder_hidden_states, dt)
         if pab_mgr.enable_pab() and ts_int is None:
             ts_int = int(timestep[0])
         if all_timesteps is not None and torch.is_tensor(all_timesteps):
@@ -227,9 +182,7 @@ class LatteT2V(nn.Module):
             Fr = x.shape[1]
         x = self._stack[0](x, enc, t6, tpe, ts_int=ts_int, all_timesteps=all_timesteps, sp_group=pm.sp_group if sp else None,
                            rope=rope, enc_lens=lens)
-        tab6 = torch.cat([self.scale_shift_table, self.scale_shift_table.new_zeros(4, C)], 0)
-        mod = K.modulation_table(tab6, torch.cat([embedded, embedded, embedded.new_zeros(B, 4 * C)], 1).contiguous(), None)
-        y = K.ln_modulate(x.view(B, Fr * S, C), mod, None, 0, 1, B, Fr, S, eps=self.eps)
+        y = ada_norm_single_out(self.scale_shift_table, embedded, x.view(B, Fr * S, C), B, Fr, S, self.eps)
         y = K.gemm_bias_act(y, self.proj_out.weight, self.proj_out.bias)  # [B, F*S, p*p*Cout]
         if sp:
             y = comm.gather_sequence(y.view(B, Fr, S, -1), pm.sp_group, dim=1, pad=comm.get_pad("temporal"))

@@ -17,27 +17,16 @@ State-dict compatible with the reference / HF ``LanguageBind/Open-Sora-Plan-v1.2
 attention down-sampler and conv feed-forward are not built).  Pinned against the reference file executed unmodified
 (tests/test_oracle_vs_reference.py::test_osp_v120_*; diffusers leaves = the reference's vendored copies).
 """
-import math
-
 import torch
 import torch.nn as nn
-import torch.nn.functional as F
 
 from ... import kernels
 from ...core.distributed import comm
-from ...core.distributed.parallel_mgr import ParallelManager
 from ...core.pab import pab_mgr
-from .latte_transformer_3d import _AdaLNSingle, _Attn, _FF, _PatchEmbed2D, _sincos_1d
-
-
-def _grid(n, base, scale):
-    return torch.arange(n, dtype=torch.float32) / (n / base) / scale
-
-
-def pos_embed_2d(embed_dim, hw, base_hw, scale_hw):
-    """reference get_2d_sincos_pos_embed :163-199 (w first)."""
-    grid_w, grid_h = torch.meshgrid(_grid(hw[1], base_hw[1], scale_hw[1]), _grid(hw[0], base_hw[0], scale_hw[0]), indexing="xy")
-    return torch.cat([_sincos_1d(embed_dim // 2, grid_w), _sincos_1d(embed_dim // 2, grid_h)], dim=1).float()
+from ._attention import apply_rope_, cross_attention, packed_self_attention, ulysses_attention
+from ._common import (AdaLNSingle, Lin2, PatchEmbed2D, ada_norm_single, ada_norm_single_out, fused_linear, grid_1d,
+                      parallel_manager, pos_embed_2d, sincos_1d, text_lens)
+from .latte_transformer_3d import _Attn, _FF
 
 
 def rope3d_tables(head_dim, t, h, w, scales_thw, dtype, device):
@@ -63,15 +52,6 @@ def rope3d_tables(head_dim, t, h, w, scales_thw, dtype, device):
     return torch.cat(cs, -1).contiguous().to(device), torch.cat(sn, -1).contiguous().to(device), half
 
 
-class _TextProjection(nn.Module):
-    """PixArtAlphaTextProjection(in_features, hidden_size, act_fn='gelu_tanh')."""
-
-    def __init__(self, cin, dim):
-        super().__init__()
-        self.linear_1 = nn.Linear(cin, dim)
-        self.linear_2 = nn.Linear(dim, dim)
-
-
 class OSPBlock(nn.Module):
     def __init__(self, dim, cross_dim, bias=True):
         super().__init__()
@@ -82,16 +62,6 @@ class OSPBlock(nn.Module):
         self._fused = {}
         self.spatial_count = self.cross_count = 0
         self.spatial_last = self.cross_last = None
-
-    def fused(self, which):
-        a = self.attn1 if which == "qkv" else self.attn2
-        mods = (a.to_q, a.to_k, a.to_v) if which == "qkv" else (a.to_k, a.to_v)
-        key = tuple((m.weight.data_ptr(), m.weight._version, m.weight.dtype) for m in mods)
-        c = self._fused.get(which)
-        if c is None or c[0] != key:
-            c = self._fused[which] = (key, torch.cat([m.weight for m in mods], 0).contiguous(),
-                                      torch.cat([m.bias for m in mods], 0).contiguous())
-        return c[1], c[2]
 
 
 class OpenSoraT2V(nn.Module):
@@ -122,18 +92,18 @@ class OpenSoraT2V(nn.Module):
         self.scale_t = interpolation_scale_t if interpolation_scale_t is not None else st
         self.scale_hw = (interpolation_scale_h if interpolation_scale_h is not None else sample_size[0] / 30,
                          interpolation_scale_w if interpolation_scale_w is not None else sample_size[1] / 40)
-        self.pos_embed = _PatchEmbed2D(patch_size, in_channels, dim)
+        self.pos_embed = PatchEmbed2D(patch_size, in_channels, dim)
         self._grid_hw = (sample_size[0] // patch_size, sample_size[1] // patch_size)
         self.num_frames = (sample_size_t - 1) // patch_size_t + 1 if sample_size_t % 2 == 1 else sample_size_t // patch_size_t
         if not use_rope:  # PatchEmbed2D(use_abs_pos=True) :270-283
             self.register_buffer("pos_table", pos_embed_2d(dim, self._grid_hw, self._grid_hw, self.scale_hw)[None], persistent=False)
-            tpe = _sincos_1d(dim, _grid(self.num_frames, self.num_frames, self.scale_t))
+            tpe = sincos_1d(dim, grid_1d(self.num_frames, self.num_frames, self.scale_t))
             self.register_buffer("temp_pos_embed", tpe.float()[None], persistent=False)
         self.transformer_blocks = nn.ModuleList([OSPBlock(dim, cross_attention_dim) for _ in range(num_layers)])
         self.scale_shift_table = nn.Parameter(torch.randn(2, dim) / dim**0.5)
         self.proj_out = nn.Linear(dim, patch_size_t * patch_size * patch_size * out_channels)
-        self.adaln_single = _AdaLNSingle(dim)
-        self.caption_projection = _TextProjection(caption_channels, dim)
+        self.adaln_single = AdaLNSingle(dim)
+        self.caption_projection = Lin2(caption_channels, dim)  # PixArtAlphaTextProjection(act_fn='gelu_tanh')
         self._rope = {}
         self.parallel_manager = None
 
@@ -146,37 +116,12 @@ class OpenSoraT2V(nn.Module):
 
     def enable_parallel(self, dp_size=None, sp_size=None, enable_cp=None):
         """Reference :1688-1700 (the forward never uses the cp group)."""
-        dp_size, sp_size = dp_size or 1, sp_size or 1
-        cp_size = 1
-        if enable_cp and sp_size % 2 == 0:
-            sp_size, cp_size = sp_size // 2, 2
-        if self.config.num_attention_heads % sp_size:
-            raise ValueError(f"Number of heads {self.config.num_attention_heads} must be divisible by sequence parallel size {sp_size}")
-        self.parallel_manager = ParallelManager(dp_size, cp_size, sp_size)
+        self.parallel_manager = parallel_manager(dp_size, sp_size, enable_cp, self.config.num_attention_heads)
 
     def reset_pab_state(self):
         for b in self.transformer_blocks:
             b.spatial_count = b.cross_count = 0
             b.spatial_last = b.cross_last = None
-
-    @staticmethod
-    def _time_proj(timesteps, dim=256):
-        half = dim // 2
-        exponent = -math.log(10000.0) * torch.arange(half, dtype=torch.float32, device=timesteps.device) / half
-        emb = timesteps[:, None].float() * exponent.exp()[None]
-        return torch.cat([emb.cos(), emb.sin()], dim=-1)
-
-    @staticmethod
-    def _text_lens(mask, B, L):
-        if mask is None:
-            return None
-        m = mask.reshape(B, -1)[:, -L:].to(torch.bool).cpu()
-        lens = m.sum(-1)
-        if not torch.equal(m, torch.arange(L)[None] < lens[:, None]):
-            raise NotImplementedError("videosys_b200: the text mask must keep a prefix of the tokens (tokenizer padding)")
-        if int(lens.min()) == 0:
-            raise NotImplementedError("videosys_b200: a sample with no valid text token")
-        return [int(v) for v in lens]
 
     def _rope_for(self, T, h, w, dtype, device):
         key = (T, h, w, dtype, str(device))
@@ -198,22 +143,14 @@ class OpenSoraT2V(nn.Module):
             a = blk.spatial_last
         else:
             xm = K.ln_modulate(x, mod, None, 0, 1, B, 1, N, eps=self.eps)
-            w, bias = blk.fused("qkv")
-            qkv = K.gemm_bias_act(xm.view(B * N, C), w, bias)
+            a1 = blk.attn1
+            qkv = K.gemm_bias_act(xm.view(B * N, C), *fused_linear(blk._fused, a1.to_q, a1.to_k, a1.to_v))
             if sp_group is None:
                 if rope is not None:
-                    K.qk_rope_halves_(qkv, rope[0], rope[1], H, D, rope[2], pos_div=1, pos_mod=N)
-                q3 = qkv.view(B * N, 3, C)
-                o = K.attn_flash(q3[:, 0], q3[:, 1], q3[:, 2], B, N, N, H, D, 3 * C, N * 3 * C, 3 * C, N * 3 * C, D**-0.5)
+                    apply_rope_(qkv, rope, H, D, pos_div=1, pos_mod=N)
+                o = packed_self_attention(qkv, B, N, H, D, D**-0.5)
             else:  # tokens for heads (:907-911): every token, H / sp heads; RoPE on the full sequence; back (:937-940)
-                full = comm.ulysses_scatter_heads(qkv.view(B, N, 3, H, D), 0, sp_group).contiguous()
-                Hn = full.shape[3]
-                Cn = Hn * D
-                if rope is not None:
-                    K.qk_rope_halves_(full, rope[0], rope[1], Hn, D, rope[2], pos_div=1, pos_mod=Ng)
-                f3 = full.view(B * Ng, 3, Cn)
-                of = K.attn_flash(f3[:, 0], f3[:, 1], f3[:, 2], B, Ng, Ng, Hn, D, 3 * Cn, Ng * 3 * Cn, 3 * Cn, Ng * 3 * Cn, D**-0.5)
-                o = comm.ulysses_gather_heads(of.view(B, Ng, Cn), 0, sp_group).contiguous()
+                o = ulysses_attention(qkv.view(B, N, 3, H, D), 0, Ng, sp_group, D**-0.5, rope=rope)
             a = K.gemm_bias_act(o.view(B * N, C), blk.attn1.to_out[0].weight, blk.attn1.to_out[0].bias)
             if pab_on:
                 blk.spatial_last = a
@@ -227,9 +164,8 @@ class OpenSoraT2V(nn.Module):
         else:
             a2 = blk.attn2
             q = K.gemm_bias_act(x.view(B * N, C), a2.to_q.weight, a2.to_q.bias)
-            wkv, bkv = blk.fused("kv")
-            kv = K.gemm_bias_act(enc2, wkv, bkv).view(-1, 2, C)
-            o = K.attn_flash(q, kv[:, 0], kv[:, 1], B, N, L, H, D, C, N * C, 2 * C, L * 2 * C, D**-0.5, kv_lens=lens)
+            kv = K.gemm_bias_act(enc2, *fused_linear(blk._fused, a2.to_k, a2.to_v)).view(-1, 2, C)
+            o = cross_attention(q, kv, B, N, L, H, D, D**-0.5, kv_lens=lens)
             xc = K.gemm_bias_act(o.view(B * N, C), a2.to_out[0].weight, a2.to_out[0].bias)
             if pab_on:
                 blk.cross_last = xc
@@ -262,7 +198,7 @@ class OpenSoraT2V(nn.Module):
         h, w = Hh // p, Ww // p
         S = h * w
         L = encoder_hidden_states.shape[1]
-        lens = self._text_lens(encoder_attention_mask, B, L)
+        lens = text_lens(encoder_attention_mask, B, L)
         x = hidden_states.to(dt).permute(0, 2, 1, 3, 4).reshape(B * Fr, Cin, Hh, Ww)
         x = self.pos_embed.proj(x).flatten(2).transpose(1, 2)  # conv: cuDNN (glue, once per step); [B*F, S, C]
         if not self.use_rope:
@@ -272,14 +208,7 @@ class OpenSoraT2V(nn.Module):
             x = (x + pos.to(x.dtype)).to(dt).view(B, Fr, S, C)
             x = (x + self.temp_pos_embed.to(dt).unsqueeze(2)).to(dt)
         x = x.reshape(B, Fr * S, C).contiguous()
-        te = self.adaln_single.emb.timestep_embedder
-        t_emb = self._time_proj(timestep).to(dt)
-        embedded = K.gemm_bias_act(F.silu(K.gemm_bias_act(t_emb, te.linear_1.weight, te.linear_1.bias)), te.linear_2.weight,
-                                   te.linear_2.bias)  # [B, C]
-        t6 = K.gemm_bias_act(F.silu(embedded), self.adaln_single.linear.weight, self.adaln_single.linear.bias)  # [B, 6C]
-        cp = self.caption_projection
-        enc = K.gemm_bias_act(K.gemm_bias_act(encoder_hidden_states.to(dt).contiguous(), cp.linear_1.weight, cp.linear_1.bias, act=1),
-                              cp.linear_2.weight, cp.linear_2.bias)  # [B, L, C]
+        embedded, t6, enc = ada_norm_single(self.adaln_single, self.caption_projection, timestep, encoder_hidden_states, dt)
         enc2 = enc.reshape(B * L, C).contiguous()
         if pab_mgr.enable_pab() and ts_int is None:
             ts_int = int(timestep[0])
@@ -291,9 +220,7 @@ class OpenSoraT2V(nn.Module):
         for blk in self.transformer_blocks:
             mod = K.modulation_table(blk.scale_shift_table, t6, None)
             self._run_block(blk, x, enc2, mod, B, N, Ng, L, lens, rope, ts_int, sp_group)
-        tab6 = torch.cat([self.scale_shift_table, self.scale_shift_table.new_zeros(4, C)], 0)
-        mod = K.modulation_table(tab6, torch.cat([embedded, embedded, embedded.new_zeros(B, 4 * C)], 1).contiguous(), None)
-        y = K.ln_modulate(x, mod, None, 0, 1, B, 1, N, eps=1e-6)
+        y = ada_norm_single_out(self.scale_shift_table, embedded, x, B, 1, N, 1e-6)
         y = K.gemm_bias_act(y.view(B * N, C), self.proj_out.weight, self.proj_out.bias).view(B, N, -1)
         if sp_group is not None:  # the head is row-wise: gather its narrow output (the reference gathers the C-wide rows, :1944-1948)
             y = comm.gather_sequence(y, sp_group, dim=1)

@@ -29,6 +29,8 @@ from ... import kernels
 from ...core.distributed import comm
 from ...core.distributed.parallel_mgr import ParallelManager
 from ...core.pab import pab_mgr
+from ._attention import cross_attention, packed_self_attention, temporal_attention
+from ._common import parallel_manager, timestep_sinusoid
 
 
 class STDiT3Config:
@@ -156,13 +158,6 @@ class _Rope(nn.Module):
         self.freqs = nn.Parameter(1.0 / (theta ** (torch.arange(0, dim, 2)[: dim // 2].float() / dim)), requires_grad=False)
 
 
-def _sinusoid(t: torch.Tensor, dim: int = 256) -> torch.Tensor:
-    half = dim // 2
-    f = torch.exp(-math.log(10000.0) * torch.arange(half, dtype=torch.float32, device=t.device) / half)
-    a = t[:, None].float() * f[None]
-    return torch.cat([a.cos(), a.sin()], dim=-1)
-
-
 class STDiT3(nn.Module):
     config_class = STDiT3Config
 
@@ -201,10 +196,6 @@ class STDiT3(nn.Module):
         # DSP switch fused into its producer / consumer (ln_modulate stores to the peers, gate+residual pulls from
         # them); VSB_DSP_FUSED=0 selects the standalone scatter kernel (vsb_dsp_scatter)
         self._fuse_dsp = os.environ.get("VSB_DSP_FUSED", "1") == "1"
-        # gate/residual inside the proj / fc2 GEMM epilogue (vsb_gemm_bias_residual): one pass over the residual
-        # instead of GEMM + gate_residual, and 168 fewer launches per step.  VSB_FUSE_EPILOGUE=0 restores the separate
-        # one-pass kernels.
-        self._fuse_epilogue = os.environ.get("VSB_FUSE_EPILOGUE", "1") == "1"
 
     # ------------------------------------------------------------------------------------------------------
     def initialize_weights(self):
@@ -231,13 +222,7 @@ class STDiT3(nn.Module):
         return build_from_pretrained(cls, path, subfolder, config_cls=STDiT3Config, **config_overrides)
 
     def enable_parallel(self, dp_size=None, sp_size=None, enable_cp=None, parallel_mgr=None):
-        if parallel_mgr is not None:
-            self.parallel_manager = parallel_mgr
-        else:
-            cp_size = 1
-            if enable_cp and sp_size % 2 == 0:
-                sp_size, cp_size = sp_size // 2, 2
-            self.parallel_manager = ParallelManager(dp_size, cp_size, sp_size)
+        self.parallel_manager = parallel_mgr if parallel_mgr is not None else parallel_manager(dp_size, sp_size, enable_cp)
         for blk in [*self.spatial_blocks, *self.temporal_blocks]:
             blk.parallel_manager = self.parallel_manager
 
@@ -275,7 +260,7 @@ class STDiT3(nn.Module):
         return self._rope_cache[key]
 
     def _embed(self, emb: _Embed2, v: torch.Tensor, dtype) -> torch.Tensor:
-        return emb.mlp(_sinusoid(v).to(dtype))
+        return emb.mlp(timestep_sinusoid(v).to(dtype))
 
     def encode_text(self, y, mask=None):
         """Reference STDiT3.encode_text (:526-537): caption MLP, then the mask-compacted [1, sum(lens), C] layout."""
@@ -372,26 +357,6 @@ class STDiT3(nn.Module):
                                            scatter_pad=comm.get_pad("temporal"), gather_pad=comm.get_pad("spatial"))
         return out.contiguous()  # the narrow() that drops the padding leaves a strided view
 
-    def _temporal_attention(self, qkv, wq, wk, B, T, S, H, D, device):
-        """Temporal self-attention on the token-major [B, T, S] activation (no rearrange): sequences of T frames per
-        (sample, patch).  T < 30: native_attention semantics in one kernel (attentions.py:95-97,111-120).  T >= 30: the
-        reference takes F.scaled_dot_product_attention (attentions.py:98-100) -> RMSNorm + RoPE pre-pass, then the flash
-        kernel over strided views (batch = patch, row = frame), one launch per sample."""
-        K = kernels
-        C = H * D
-        cos, sin = self._rope_tables(T, device)
-        if T < 30:
-            return K.attn_short(qkv.view(-1, 3, H, D), wq, wk, cos, sin, B, S, T * S, 1, S, T, H, D, D**-0.5)
-        if S > 65535:
-            raise RuntimeError("temporal flash attention: more than 65535 patches per frame")
-        K.qk_rmsnorm_(qkv, wq, wk, H, D, rope_cos=cos, rope_sin=sin, pos_div=S, pos_mod=T)
-        o = torch.empty(B * T * S, C, dtype=qkv.dtype, device=device)
-        q3 = qkv.view(B, T * S, 3, C)
-        for b in range(B):
-            K.attn_flash(q3[b, :, 0], q3[b, :, 1], q3[b, :, 2], S, T, T, H, D, S * 3 * C, 3 * C, S * 3 * C, 3 * C, D**-0.5,
-                         out=o[b * T * S:], out_row_stride=S * C, out_batch_stride=C)
-        return o
-
     def _run_block(self, blk: STDiT3Block, x, text, t_mlp, t0_mlp, mask_u8, B, T, S, Tg, Sg, plan=(False, False)):
         """x: [B, T*S, C] resident layout (T full, S local); Tg/Sg are the global extents (== T, S when sp == 1).
         text: the dict of _text_state; plan: (reuse_attn, reuse_cross) of this block for this step."""
@@ -416,7 +381,9 @@ class STDiT3(nn.Module):
             if blk.temporal:
                 xm = K.ln_modulate(x, mod, mask_u8, 0, 1, B, T, S)
                 qkv = K.gemm_bias_act(xm, a.qkv.weight, a.qkv.bias)
-                o = self._temporal_attention(qkv, wq, wk, B, T, S, H, D, x.device)
+                # T < 30: native_attention semantics in one kernel (attentions.py:95-97,111-120); T >= 30: the reference
+                # takes F.scaled_dot_product_attention (attentions.py:98-100), same softmax on the flash kernel
+                o = temporal_attention(qkv, B, T, S, H, D, D**-0.5, 29, wq, wk, rope=self._rope_tables(T, x.device))
             else:
                 Ba = B
                 if fused_dsp:
@@ -441,19 +408,13 @@ class STDiT3(nn.Module):
                     xm = K.ln_modulate(x, mod, mask_u8, 0, 1, B, T, S)
                     Ta, Sa = T, S
                 qkv = K.gemm_bias_act(xm, a.qkv.weight, a.qkv.bias)
-                if Sa >= 30:
-                    K.qk_rmsnorm_(qkv, wq, wk, H, D)
-                    q3 = qkv.view(-1, 3, C)
-                    o = K.attn_flash(q3[:, 0], q3[:, 1], q3[:, 2], Ba * Ta, Sa, Sa, H, D, 3 * C, Sa * 3 * C, 3 * C,
-                                     Sa * 3 * C, D**-0.5)
-                else:
-                    o = K.attn_short(qkv.view(-1, 3, H, D), wq, wk, None, None, Ba * Ta, 1, Sa, 0, 1, Sa, H, D, D**-0.5)
+                o = packed_self_attention(qkv, Ba * Ta, Sa, H, D, D**-0.5, short_max=29, wq=wq, wk=wk)
             cache = None
             if pab_on:
                 if blk.last_attn is None or blk.last_attn.shape != x.shape:
                     blk.last_attn = torch.empty_like(x)
                 cache = blk.last_attn
-            if self._fuse_epilogue and not pab_on and (blk.temporal or sp == 1):
+            if not pab_on and (blk.temporal or sp == 1):
                 # gate + select + residual in the proj GEMM's epilogue (no PAB cache to fill, no reshard in between)
                 K.gemm_bias_residual(o.view(-1, C), a.proj.weight, a.proj.bias, x, mod, mask_u8, 2, B, T, S)
             elif fused_dsp:
@@ -480,27 +441,18 @@ class STDiT3(nn.Module):
             if kv is None:  # timestep-independent: one kv_linear per block per prompt, not per step
                 kv = K.gemm_bias_act(text["y_tok"], c.kv_linear.weight, c.kv_linear.bias)
                 text["kv"][id(blk)] = kv
-            Lv = text["Lv"]
-            kv2 = kv.view(-1, 2, C)
-            o = K.attn_flash(q, kv2[:, 0], kv2[:, 1], B, T * S, Lv, H, D, C, T * S * C, 2 * C, Lv * 2 * C, D**-0.5,
-                             kv_lens=text["kv_lens"])
-            if self._fuse_epilogue and not pab_on:
+            o = cross_attention(q, kv.view(-1, 2, C), B, T * S, text["Lv"], H, D, D**-0.5, kv_lens=text["kv_lens"])
+            if not pab_on:
                 K.gemm_bias_residual(o.view(-1, C), c.proj.weight, c.proj.bias, x)  # x += proj(o) in the epilogue
-            else:
-                out = blk.last_cross if (pab_on and blk.last_cross is not None and blk.last_cross.shape == x.shape) else None
-                xc = K.gemm_bias_act(o, c.proj.weight, c.proj.bias, out=out)
-                if pab_on:
-                    blk.last_cross = xc
-                K.residual_add(x, xc.view(x.shape), out=x)
+            else:  # PAB: the branch is cached for the steps that reuse it
+                out = blk.last_cross if (blk.last_cross is not None and blk.last_cross.shape == x.shape) else None
+                blk.last_cross = K.gemm_bias_act(o, c.proj.weight, c.proj.bias, out=out)
+                K.residual_add(x, blk.last_cross.view(x.shape), out=x)
 
         # ---- MLP ----
         xm = K.ln_modulate(x, mod, mask_u8, 3, 4, B, T, S)
         h = K.gemm_bias_act(xm, blk.mlp.fc1.weight, blk.mlp.fc1.bias, act=1)
-        if self._fuse_epilogue:
-            K.gemm_bias_residual(h.view(-1, h.shape[-1]), blk.mlp.fc2.weight, blk.mlp.fc2.bias, x, mod, mask_u8, 5, B, T, S)
-        else:
-            y = K.gemm_bias_act(h, blk.mlp.fc2.weight, blk.mlp.fc2.bias)
-            K.gate_residual(x, y, mod, mask_u8, 5, B, T, S, out=x)
+        K.gemm_bias_residual(h.view(-1, h.shape[-1]), blk.mlp.fc2.weight, blk.mlp.fc2.bias, x, mod, mask_u8, 5, B, T, S)
         return x
 
     # ---- STDiT3.forward --------------------------------------------------------------------------------------
@@ -573,7 +525,7 @@ class STDiT3(nn.Module):
             s_pad = comm.get_pad("spatial")
         Sl = (S + s_pad) // sp
         h = None
-        if p[0] == 1 and os.environ.get("VSB_PATCH_EMBED", "1") != "0":
+        if p[0] == 1:
             proj = self.x_embedder.proj
             h = kernels.patch_embed(x.contiguous(), proj.weight, proj.bias, pos.reshape(S, C), p[1], p[2],
                                     s0=(pm.sp_rank * Sl if sp > 1 else 0), s_local=Sl)

@@ -31,36 +31,18 @@ against the reference's attention class + processor bit for bit.
 The reference pipeline calls the transformer with batch 1 (pipeline_vchitect.py:925-941); with a larger batch its
 ``temb.repeat(F, 1)`` pairs frames with the wrong sample's conditioning, so batch > 1 is rejected here.
 """
-import math
-
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
 from ... import kernels
 from ...core.distributed import comm
-from ...core.distributed.parallel_mgr import ParallelManager
 from ...core.pab import pab_mgr
+from ._attention import cross_attention, packed_self_attention, temporal_attention
+from ._common import fused_linear, parallel_manager, pos_embed_2d, timestep_sinusoid
 
 
 # ---- diffusers pieces, restated -----------------------------------------------------------------------------------------
-def _sincos_1d(embed_dim: int, pos: torch.Tensor) -> torch.Tensor:
-    """get_1d_sincos_pos_embed_from_grid: [sin(pos w) | cos(pos w)], w_i = 10000^(-i / (embed_dim/2)), float64."""
-    omega = 1.0 / 10000 ** (torch.arange(embed_dim // 2, dtype=torch.float64) / (embed_dim / 2.0))
-    out = pos.reshape(-1).double()[:, None] * omega[None]
-    return torch.cat([out.sin(), out.cos()], dim=1)
-
-
-def get_2d_sincos_pos_embed(embed_dim: int, grid_size: int, base_size: int = 16, interpolation_scale: float = 1.0):
-    """diffusers.models.embeddings.get_2d_sincos_pos_embed (0.30.0): [grid_size**2, embed_dim] float32; the first half of
-    the channels encodes the w coordinate (np.meshgrid(grid_w, grid_h) puts w first), the second half h."""
-    gh = torch.arange(grid_size, dtype=torch.float32) / (grid_size / base_size) / interpolation_scale
-    gw = torch.arange(grid_size, dtype=torch.float32) / (grid_size / base_size) / interpolation_scale
-    grid_w, grid_h = torch.meshgrid(gw, gh, indexing="xy")  # both [grid, grid]: grid_w varies along columns
-    emb_h = _sincos_1d(embed_dim // 2, grid_w)  # the library calls grid[0] (= w) its "h" half
-    emb_w = _sincos_1d(embed_dim // 2, grid_h)
-    return torch.cat([emb_h, emb_w], dim=1).float()
-
 
 class _PatchEmbed(nn.Module):
     """diffusers PatchEmbed as SD3 / Vchitect use it (layer_norm False, pos_embed_max_size set -> persistent buffer)."""
@@ -70,7 +52,8 @@ class _PatchEmbed(nn.Module):
         self.proj = nn.Conv2d(in_channels, embed_dim, kernel_size=(patch_size, patch_size), stride=patch_size, bias=True)
         self.patch_size, self.pos_embed_max_size = patch_size, pos_embed_max_size
         self.base_size = height // patch_size
-        pos = get_2d_sincos_pos_embed(embed_dim, pos_embed_max_size, base_size=self.base_size)
+        m, b = pos_embed_max_size, self.base_size
+        pos = pos_embed_2d(embed_dim, (m, m), (b, b), (1.0, 1.0))
         self.register_buffer("pos_embed", pos.unsqueeze(0), persistent=True)
 
     def cropped_pos_embed(self, height, width):
@@ -102,15 +85,8 @@ class _TimeTextEmbed(nn.Module):
         self.timestep_embedder = _Lin2(256, embedding_dim)
         self.text_embedder = _Lin2(pooled_projection_dim, embedding_dim)
 
-    @staticmethod
-    def time_proj(timesteps: torch.Tensor) -> torch.Tensor:
-        half = 128
-        exponent = -math.log(10000.0) * torch.arange(half, dtype=torch.float32, device=timesteps.device) / half
-        emb = timesteps[:, None].float() * exponent.exp()[None]
-        return torch.cat([emb.cos(), emb.sin()], dim=-1)  # flip_sin_to_cos
-
     def forward(self, timestep, pooled):
-        t = self.timestep_embedder(self.time_proj(timestep).to(pooled.dtype))
+        t = self.timestep_embedder(timestep_sinusoid(timestep).to(pooled.dtype))
         return t + self.text_embedder(pooled)
 
 
@@ -162,17 +138,6 @@ class VchitectAttention(nn.Module):
         self.spatial_count = self.temporal_count = self.cross_count = 0
         self.last_spatial = self.last_temporal = self.last_cross = None
         self._fused = {}
-
-    def fused(self, *names):
-        """One [sum N, K] weight (+ bias) for several Linear layers that read the same input (rebuilt when a parameter
-        changes: load_state_dict / .to())."""
-        mods = [getattr(self, n) for n in names]
-        key = tuple((m.weight.data_ptr(), m.weight._version, m.weight.dtype) for m in mods)
-        hit = self._fused.get(names)
-        if hit is None or hit[0] != key:
-            hit = (key, torch.cat([m.weight for m in mods], 0).contiguous(), torch.cat([m.bias for m in mods], 0).contiguous())
-            self._fused[names] = hit
-        return hit[1], hit[2]
 
 
 class JointTransformerBlock(nn.Module):
@@ -234,11 +199,7 @@ class VchitectXLTransformerModel(nn.Module):
         v to a token shard holding every frame and switches the result back (processor :725-727, :758-759, :929-949; NCCL
         all-to-all).  As in the reference, ``enable_cp`` only takes a factor 2 out of sp_size: the forward never uses the cp
         group (the pipeline runs the two CFG branches one after the other)."""
-        dp_size, sp_size = dp_size or 1, sp_size or 1
-        cp_size = 1
-        if enable_cp and sp_size % 2 == 0:
-            sp_size, cp_size = sp_size // 2, 2
-        self.parallel_manager = ParallelManager(dp_size, cp_size, sp_size)
+        self.parallel_manager = parallel_manager(dp_size, sp_size, enable_cp)
 
     def reset_pab_state(self):
         for b in self.transformer_blocks:
@@ -267,8 +228,8 @@ class VchitectXLTransformerModel(nn.Module):
         dev, dt = nh.device, nh.dtype
         scale = D**-0.5
         pab_on = pab_mgr.enable_pab()
-        w, b = a.fused("add_q_proj", "add_k_proj", "add_v_proj")
-        eqkv = K.gemm_bias_act(ne.view(Fr * L, C), w, b).view(Fr, L, 3 * C)  # context projections (:823-825)
+        eqkv = K.gemm_bias_act(ne.view(Fr * L, C), *fused_linear(a._fused, a.add_q_proj, a.add_k_proj, a.add_v_proj))
+        eqkv = eqkv.view(Fr, L, 3 * C)  # context projections (:823-825)
 
         # temporal (:838-856)
         reuse = False
@@ -277,7 +238,7 @@ class VchitectXLTransformerModel(nn.Module):
         if reuse:
             hid_t, enc_t = a.last_temporal
         else:
-            w, b = a.fused("to_q_temp", "to_k_temp", "to_v_temp")
+            w, b = fused_linear(a._fused, a.to_q_temp, a.to_k_temp, a.to_v_temp)
             jt = torch.empty(Fr, N, 3 * C, dtype=dt, device=dev)
             jt[:, :S] = K.gemm_bias_act(nh.view(Fr * S, C), w, b).view(Fr, S, 3 * C)
             jt[:, S:] = eqkv
@@ -288,15 +249,7 @@ class VchitectXLTransformerModel(nn.Module):
                                               scatter_pad=comm.get_pad("spatial"), gather_pad=comm.get_pad("temporal")).contiguous()
                 Ft, Nt = jt.shape[1], jt.shape[2]
                 jt = jt.view(Ft, Nt, 3 * C)
-            cos, sin = self._rope_tables(Ft, dev)
-            if Ft <= 64:
-                ot = K.attn_short(jt.view(-1, 3, H, D), None, None, cos, sin, 1, Nt, Ft * Nt, 1, Nt, Ft, H, D, scale, flags=3)
-            else:
-                K.qk_rmsnorm_(jt, None, None, H, D, rope_cos=cos, rope_sin=sin, pos_div=Nt, pos_mod=Ft)
-                ot = torch.empty(Ft * Nt, C, dtype=dt, device=dev)
-                q3 = jt.view(Ft * Nt, 3, C)
-                K.attn_flash(q3[:, 0], q3[:, 1], q3[:, 2], Nt, Ft, Ft, H, D, Nt * 3 * C, 3 * C, Nt * 3 * C, 3 * C, scale,
-                             out=ot, out_row_stride=Nt * C, out_batch_stride=C)
+            ot = temporal_attention(jt, 1, Ft, Nt, H, D, scale, 64, rope=self._rope_tables(Ft, dev), sdpa=True)
             if sp_group is not None:  # token shard -> frame shard
                 ot = comm.all_to_all_with_pad(ot.view(1, Ft, Nt, C), sp_group, scatter_dim=1, gather_dim=2,
                                               scatter_pad=comm.get_pad("temporal"), gather_pad=comm.get_pad("spatial")).contiguous()
@@ -316,8 +269,7 @@ class VchitectXLTransformerModel(nn.Module):
             jc = torch.empty(Fr, N, C, dtype=dt, device=dev)
             jc[:, :S] = K.gemm_bias_act(nh.view(Fr * S, C), a.to_q_cross.weight, a.to_q_cross.bias).view(Fr, S, C)
             jc[:, S:] = eqkv[:, :, :C]
-            e0 = eqkv[0].view(L, 3, C)
-            oc = K.attn_flash(jc, e0[:, 1], e0[:, 2], 1, Fr * N, L, H, D, C, Fr * N * C, 3 * C, L * 3 * C, scale)
+            oc = cross_attention(jc, eqkv[0].view(L, 3, C), 1, Fr * N, L, H, D, scale)
             cross = K.gemm_bias_act(oc.view(Fr * N, C), a.to_out_context.weight, a.to_out_context.bias)
             if pab_on:
                 a.last_cross = cross
@@ -329,13 +281,11 @@ class VchitectXLTransformerModel(nn.Module):
         if reuse:
             sp_out = a.last_spatial
         else:
-            w, b = a.fused("to_q", "to_k", "to_v")
+            w, b = fused_linear(a._fused, a.to_q, a.to_k, a.to_v)
             js = torch.empty(Fr, N, 3 * C, dtype=dt, device=dev)
             js[:, :S] = K.gemm_bias_act(nh.view(Fr * S, C), w, b).view(Fr, S, 3 * C)
             js[:, S:] = eqkv
-            q3 = js.view(Fr * N, 3, C)
-            sp_out = K.attn_flash(q3[:, 0], q3[:, 1], q3[:, 2], Fr, N, N, H, D, 3 * C, N * 3 * C, 3 * C, N * 3 * C, scale)
-            sp_out = sp_out.view(Fr * N, C)
+            sp_out = packed_self_attention(js, Fr, N, H, D, scale).view(Fr * N, C)
             if pab_on:
                 a.last_spatial = sp_out
 
