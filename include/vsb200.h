@@ -38,9 +38,7 @@ unsigned long long vsb_launch_count(void);
 /* Encoded TMA tensor maps are cached by (base, shape, strides, box, swizzle): which = 0 -> hits, 1 -> misses (host
  * cuTensorMapEncodeTiled calls actually made).  Option "tmap_cache" (default 1) turns the cache off. */
 unsigned long long vsb_tmap_cache_stats(int which);
-/* Run-time kernel selection knobs (not a backend switch: every choice is an sm_90a kernel of this library).
- *   "dsp_rowwise" (default 1): vsb_dsp_scatter decodes indices once per token row; 0 = the first version (per vector).
- *   "ln_occupancy" (default 3): 4 = vsb_ln_modulate compiled for 4 resident blocks per SM (64 registers).
+/* Run-time options.
  *   "tmap_cache" (default 1): cache of encoded TMA tensor maps. */
 int vsb_set_option(const char* name, int value);
 
@@ -175,38 +173,32 @@ int vsb_attn_flash_strided(const vsb_bf16* q, const vsb_bf16* k, const vsb_bf16*
  * has_timestep = 0 models `timestep is None`. */
 int vsb_pab_gate(int broadcast_on, int has_timestep, int timestep, int* count, int range, int lo, int hi, int steps);
 
-/* ---- DSP reshard (dimension switch) over NVLink peer memory ----------------------------------------------------
+/* ---- DSP dimension switch over NVLink peer memory ---------------------------------------------------------------
  * replaces STDiT3Block.dynamic_switch -> all_to_all_with_pad -> _all_to_all_func:
  * open_sora_transformer_3d.py:288-315, core/distributed/comm.py:282-304,104-108.
- * One kernel packs each destination rank's slice and stores it straight into that rank's receive window with
- * 128-bit peer stores (no staging copies, zero padding synthesised on the fly), then signals a per-peer flag.
- *   peer_recv[r]   device pointer (peer-mapped) to rank r's receive window for this direction
- *   peer_flags[r]  device pointer (peer-mapped) to rank r's flag array [world] (uint32 epoch counters)
- *   to_spatial_shard = 0: local [B, T, Sl, C] (S-sharded) -> recv [B, Tp/sp, Sp, C] (T-sharded)
- *   to_spatial_shard = 1: local [B, Tl, S(+pad), C] -> recv [B, Tp, Sl, C]
- * vsb_dsp_wait blocks the stream until all `world` peers have delivered epoch `epoch`. */
-int vsb_dsp_scatter(const vsb_bf16* local, void* const* host_peer_recv, void* const* host_peer_flags, int rank,
-                    int world, int to_spatial_shard, int B, int T, int S, int C, unsigned epoch, void* stream);
-int vsb_dsp_wait(void* my_flags, int world, unsigned epoch, void* stream);
-/* epoch == 0 (both calls above and below): take the next value of a DEVICE-side counter kept in the flag array
- * (slots 32 = sent, 33 = waited), so a captured CUDA graph of a whole denoising step advances the epochs on every
- * replay without host involvement.  Do not mix explicit and device-side epochs on one flag array.
+ * The switch is fused into its producer and its consumer (north_star: "in-kernel sequence-dim all-to-all issuing P2P
+ * stores fused with the preceding [producer]"; in STDiT3 the producer of the S-shard -> T-shard switch is the AdaLN
+ * modulate, open_sora_transformer_3d.py:196-216, and the consumer of the switch back is the gate + residual, :213-228):
  *
- * Producer- / consumer-fused forms of the same switch (north_star: "in-kernel sequence-dim all-to-all issuing P2P stores
- * fused with the preceding [producer]"; in STDiT3 the producer of the S-shard -> T-shard switch is the AdaLN modulate,
- * open_sora_transformer_3d.py:196-216, and the consumer of the switch back is the gate + residual, :213-228):
- *
- * vsb_ln_modulate_dsp = vsb_ln_modulate whose store path IS the reshard: row (b, t, sl) goes to peer (b*T+t) / Tl,
+ * vsb_ln_modulate_dsp = vsb_ln_modulate whose store path IS the switch: row (b, t, sl) goes to peer (b*T+t) / Tl,
  *   window viewed as [Tl, Sg, C], row ((b*T+t) % Tl, rank*Sl + sl), Tl = ceil(B*T / world) ((batch, frame) sequences
  *   are scattered, not frames: 2*20 = 40 split 8 ways exactly); zero rows for padded sequences, padded columns never
- *   sent; publishes the epoch like vsb_dsp_scatter.  Follow with vsb_dsp_wait on the same flag array.
+ *   sent; the last CTA to finish publishes the epoch into every peer's flag array.  Follow with vsb_dsp_wait on the
+ *   same flag array.
+ *     host_peer_recv[r]   device pointer (peer-mapped) to rank r's receive window
+ *     host_peer_flags[r]  device pointer (peer-mapped) to rank r's flag array (uint32 epoch counters)
  * vsb_dsp_signal publishes the next epoch without moving data (the proj GEMM wrote into this rank's OWN window).
+ * vsb_dsp_wait blocks the stream until all `world` peers have published epoch `epoch` into my_flags.
  * vsb_gate_residual_dsp = vsb_gate_residual whose y operand is PULLED with 128-bit peer loads from the producers'
- *   windows host_peer_y[r] (each viewed as [Tl, Sg, C]); call after vsb_dsp_wait on the signalled flag array. */
+ *   windows host_peer_y[r] (each viewed as [Tl, Sg, C]); call after vsb_dsp_wait on the signalled flag array.
+ * epoch == 0: take the next value of a DEVICE-side counter kept in the flag array (slots 32 = sent, 33 = waited), so a
+ * captured CUDA graph of a whole denoising step advances the epochs on every replay without host involvement.  Do not
+ * mix explicit and device-side epochs on one flag array. */
 int vsb_ln_modulate_dsp(const vsb_bf16* x, const vsb_bf16* mod, const uint8_t* x_mask, int shift_row, int scale_row,
                         int B, int T, int Sl, int C, float eps, void* const* host_peer_recv, void* const* host_peer_flags,
                         int rank, int world, int Sg, unsigned epoch, void* stream);
 int vsb_dsp_signal(void* const* host_peer_flags, int rank, int world, unsigned epoch, void* stream);
+int vsb_dsp_wait(void* my_flags, int world, unsigned epoch, void* stream);
 int vsb_gate_residual_dsp(const vsb_bf16* x, void* const* host_peer_y, vsb_bf16* out, vsb_bf16* cache_out,
                           const vsb_bf16* mod, const uint8_t* x_mask, int gate_row, int B, int T, int Sl, int C, int rank,
                           int world, int Sg, void* stream);

@@ -30,7 +30,6 @@ SIGNATURES = {
     "vsb_gemm_bias_residual": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "vsb_attn_flash": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _ll, _ll, _ll, _ll, C.POINTER(_i), _f, _vp]),
     "vsb_pab_gate": (_i, [_i, _i, _i, C.POINTER(_i), _i, _i, _i, _i]),
-    "vsb_dsp_scatter": (_i, [_vp, C.POINTER(_vp), C.POINTER(_vp), _i, _i, _i, _i, _i, _i, _i, _u, _vp]),
     "vsb_dsp_wait": (_i, [_vp, _i, _u, _vp]),
     "vsb_dsp_signal": (_i, [C.POINTER(_vp), _i, _i, _u, _vp]),
     "vsb_ln_modulate_dsp": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _f, C.POINTER(_vp), C.POINTER(_vp), _i, _i, _i, _u,

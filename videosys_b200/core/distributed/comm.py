@@ -6,11 +6,13 @@ split/gather_from_second_dim :307-318), inference only (no autograd functions); 
 ``ulysses_gather_heads`` are CogVideoX's head-scatter exchange on the packed qkv (cogvideox_transformer_3d.py:44-165).
 
 Two transports for the dimension switch:
-  * ``DspP2P`` (native path): one sm_90a kernel stores every 16-byte vector straight into the destination rank's
-    receive window over NVLink (CUDA-IPC mapped peer memory), flags + a wait kernel order the streams; no staging
-    copies, no NCCL launch (csrc/dsp_p2p.cu, C-ABI vsb_dsp_scatter / vsb_dsp_wait).
+  * ``DspP2P`` (native path): the switch is fused into its producer and consumer kernels.  The modulate kernel stores
+    its rows straight into the owners' receive windows over NVLink (CUDA-IPC mapped peer memory), and the gate +
+    residual kernel loads the branch back from the peers' windows; flags + a wait kernel order the streams; no staging
+    copies, no NCCL launch (csrc/elementwise.cu, csrc/dsp_p2p.cu; C-ABI vsb_ln_modulate_dsp / vsb_gate_residual_dsp /
+    vsb_dsp_signal / vsb_dsp_wait).
   * ``torch.distributed.all_to_all_single`` (NCCL on GPU, gloo on CPU for the host-logic tests): the fallback
-    north_star allows "where the fused P2P kernel is not taken".
+    north_star allows "where the fused P2P kernel is not taken", and the only transport where CUDA IPC is unavailable.
 """
 import ctypes as C
 from typing import Dict, List, Optional
@@ -142,10 +144,11 @@ def ulysses_gather_heads(o: torch.Tensor, n_text: int, process_group) -> torch.T
 class DspP2P:
     """Symmetric receive windows + flags for the P2P dimension switch (one instance per process / sp group).
 
-    ``switch(x, T, S, to_spatial_shard)`` is the native replacement of STDiT3Block.dynamic_switch
-    (open_sora_transformer_3d.py:288-315): x is the local [B, t, s, C] tensor, the result is a view of this rank's
-    receive window in the new layout.  The two directions own separate windows and flag arrays; stream order plus
-    the data dependencies of the block make one window per direction sufficient (see DESIGN.md section 5).
+    The native replacement of STDiT3Block.dynamic_switch (open_sora_transformer_3d.py:288-315):
+    ``ln_modulate_push`` is the S-shard -> T-shard switch fused into the modulate kernel, ``branch_window`` +
+    ``gate_residual_pull`` the way back fused into the gate + residual kernel.  The two directions own separate windows
+    and flag arrays; stream order plus the data dependencies of the block make one window per direction sufficient
+    (see DESIGN.md section 5).
     """
 
     def __init__(self, process_group, max_elems: int, device: torch.device):
@@ -201,26 +204,6 @@ class DspP2P:
         from ..._cuda_view import device_view
 
         return device_view(self._own[d][0], shape, torch.bfloat16, self.device)
-
-    def switch(self, x: torch.Tensor, T: int, S: int, to_spatial_shard: bool) -> torch.Tensor:
-        """x: local [B, T, Sl, C] (to_spatial_shard=False) or [B, Tl, S, C] (True); T, S are GLOBAL extents."""
-        d = 1 if to_spatial_shard else 0
-        B, Cc = x.shape[0], x.shape[-1]
-        w = self.world
-        Tl, Sl = -(-T // w), -(-S // w)
-        out_shape = (B, T, Sl, Cc) if to_spatial_shard else (B, Tl, S, Cc)
-        st = torch.cuda.current_stream().cuda_stream
-        from ... import kernels
-
-        # algorithmic bytes = what leaves this rank (the (w-1)/w of the local tensor that other ranks own)
-        with kernels._Timed("dsp_switch", x.numel() * 2 * (w - 1) // w):
-            self._libmod.check(
-                self.lib.vsb_dsp_scatter(x.data_ptr(), self._recv_arr[d], self._flag_arr[d], self.rank, w, d, B, T, S,
-                                         Cc, 0, st),
-                "dsp_scatter",
-            )
-            self._libmod.check(self.lib.vsb_dsp_wait(self._own[d][1], w, 0, st), "dsp_wait")
-        return self._window(d, out_shape)
 
     # ---- producer- / consumer-fused switch (csrc/elementwise.cu: ln_modulate_kernel<.., true>, gate_residual_dsp_kernel)
     def ln_modulate_push(self, x, mod, mask_u8, shift_row: int, scale_row: int, B: int, T: int, Sl: int, Sg: int,

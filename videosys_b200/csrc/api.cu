@@ -8,8 +8,6 @@
 
 namespace vsbs {
 thread_local char g_err[512] = "";
-int g_opt_dsp_rowwise = 1;    // 0: the first (per-vector) reshard kernel
-int g_opt_ln_occupancy = 3;   // ln_modulate: resident 256-thread blocks per SM the kernel is compiled for (3 or 4)
 std::atomic<unsigned long long> g_launches{0};
 static EncodeTiledFn g_encode = nullptr;
 static int g_sms = 0;
@@ -152,14 +150,6 @@ extern "C" int vsb_set_option(const char* name, int value) {
   if (!name) return fail(VSB_ERR_INVALID, "set_option: null name");
   if (!strcmp(name, "tmap_cache")) {
     g_opt_tmap_cache = value;
-    return VSB_OK;
-  }
-  if (!strcmp(name, "dsp_rowwise")) {
-    g_opt_dsp_rowwise = value;
-    return VSB_OK;
-  }
-  if (!strcmp(name, "ln_occupancy")) {
-    g_opt_ln_occupancy = value;
     return VSB_OK;
   }
   return fail(VSB_ERR_INVALID, "set_option: unknown option '%s'", name);

@@ -1,5 +1,5 @@
-// vsb200 -- device-side pieces shared by every kernel that talks to the DSP peer windows (dsp_p2p.cu: the standalone
-// reshard; elementwise.cu: the producer- / consumer-fused variants).
+// vsb200 -- device-side pieces shared by every kernel that talks to the DSP peer windows (dsp_p2p.cu: the signal and
+// wait kernels; elementwise.cu: the producer- / consumer-fused switch).
 #pragma once
 #include "vsb_common.cuh"
 

@@ -1,123 +1,12 @@
-// vsb200 -- Dynamic Sequence Parallelism reshard as direct 128-bit stores into the peers' receive windows
-// (NVLink 5 / NVSwitch P2P), replacing tensor_split+contiguous -> NCCL all_to_all -> cat+contiguous (+pad / narrow).
-//
-// The sender walks its local tensor once; every 16-byte vector goes straight to its final position in the
-// destination rank's output tensor (zero padding of the scattered axis is synthesised, padding of the gathered
-// axis is never sent).  Completion: every CTA fences (system scope); the last CTA to finish publishes the epoch
-// into each peer's flag slot; vsb_dsp_wait spins (acquire, system scope) on the receiver's stream.
+// vsb200 -- Dynamic Sequence Parallelism signalling and peer-window plumbing.  The switch itself is fused into its
+// producer and consumer (elementwise.cu: vsb_ln_modulate_dsp stores into the peers' receive windows,
+// vsb_gate_residual_dsp loads from them over NVLink).  Completion: every CTA of the producer fences (system scope); the
+// last CTA to finish publishes the epoch into each peer's flag slot; vsb_dsp_wait spins (acquire, system scope) on the
+// receiver's stream.
 #include "dsp_common.cuh"
 #include "vsb_host.h"
 
 namespace vsb {
-
-// option dsp_rowwise (api.cu): 1 = one warp per token row (default); 0 = the first version (decode per 16-byte vector)
-
-// dir 0: local [B, T, Sl, C] -> rank d receives frames [d*Tl, (d+1)*Tl) into [B, Tl, S, C] at columns rank*Sl + sl
-// dir 1: local [B, Tl, S, C] -> rank d receives columns [d*Sl, (d+1)*Sl) into [B, T, Sl, C] at frames rank*Tl + tl
-//
-// One warp per token row (C contiguous bf16 = C/8 vectors that all go to ONE contiguous row of ONE peer): the
-// (b, t, s) decode and the destination lookup cost a few 32-bit divisions per ROW.  The first version (below, kept as
-// dsp_rowwise=0) decoded every 16-byte vector with seven 64-bit divisions (~700 instructions per vector): it was
-// instruction-bound at 370-440 GB/s, not NVLink-bound.
-__global__ void __launch_bounds__(256) dsp_scatter_kernel(const bf16* __restrict__ local, DspPeers peers, int rank,
-                                                          int world, int dir, int B, int T, int S, int C,
-                                                          unsigned epoch) {
-  const unsigned Tp = ((T + world - 1) / world) * world, Sp = ((S + world - 1) / world) * world;
-  const unsigned Tl = Tp / world, Sl = Sp / world;
-  const int cv = C >> 3;
-  const int lane = threadIdx.x & 31;
-  const unsigned nwarps = gridDim.x * (blockDim.x >> 5);
-  const unsigned gw = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  const unsigned nrows = dir == 0 ? (unsigned)B * Tp * Sl : (unsigned)B * Tl * Sp;  // < 2^31 (checked by the launcher)
-  constexpr int U = 5;  // 16-byte vectors per lane per trip: loads first, then the (posted) peer stores
-  for (unsigned r = gw; r < nrows; r += nwarps) {
-    const uint4* src = nullptr;  // nullptr: synthesise the zero padding of the scattered axis
-    uint4* dst;
-    if (dir == 0) {
-      const unsigned sl = r % Sl, bt = r / Sl;
-      const unsigned t = bt % Tp, b = bt / Tp;
-      const unsigned col = rank * Sl + sl;
-      if (col >= (unsigned)S) continue;  // gathered-axis padding is narrowed away at the receiver: never sent
-      const unsigned d = t / Tl, tl = t - d * Tl;
-      if (t < (unsigned)T) src = reinterpret_cast<const uint4*>(local + (((size_t)b * T + t) * Sl + sl) * C);
-      dst = reinterpret_cast<uint4*>(peers.recv[d] + (((size_t)b * Tl + tl) * S + col) * C);
-    } else {
-      const unsigned col = r % Sp, btl = r / Sp;
-      const unsigned tl = btl % Tl, b = btl / Tl;
-      const unsigned tg = rank * Tl + tl;
-      if (tg >= (unsigned)T) continue;
-      const unsigned d = col / Sl, sl = col - d * Sl;
-      if (col < (unsigned)S) src = reinterpret_cast<const uint4*>(local + (((size_t)b * Tl + tl) * S + col) * C);
-      dst = reinterpret_cast<uint4*>(peers.recv[d] + (((size_t)b * T + tg) * Sl + sl) * C);
-    }
-    for (int v0 = lane; v0 < cv; v0 += 32 * U) {
-      uint4 v[U];
-#pragma unroll
-      for (int u = 0; u < U; ++u) {
-        const int vi = v0 + 32 * u;
-        v[u] = (src != nullptr && vi < cv) ? src[vi] : make_uint4(0, 0, 0, 0);
-      }
-#pragma unroll
-      for (int u = 0; u < U; ++u) {
-        const int vi = v0 + 32 * u;
-        if (vi < cv) dst[vi] = v[u];
-      }
-    }
-  }
-  dsp_publish(peers, rank, world, epoch);
-}
-
-// First version: every 16-byte vector decoded on its own.
-__global__ void __launch_bounds__(256) dsp_scatter_vec_kernel(const bf16* __restrict__ local, DspPeers peers, int rank,
-                                                              int world, int dir, int B, int T, int S, int C,
-                                                              unsigned epoch) {
-  const int Tp = ((T + world - 1) / world) * world, Sp = ((S + world - 1) / world) * world;
-  const int Tl = Tp / world, Sl = Sp / world;
-  const int cv = C >> 3;
-  const uint4 zero = make_uint4(0, 0, 0, 0);
-  constexpr int U = 4;
-  const long long nthreads = (long long)gridDim.x * blockDim.x;
-  const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  const long long total = dir == 0 ? (long long)B * Tp * Sl * cv : (long long)B * Tl * Sp * cv;
-  for (long long i0 = tid; i0 < total; i0 += nthreads * U) {
-    uint4 v[U];
-    uint4* dst[U];
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const long long i = i0 + (long long)u * nthreads;
-      dst[u] = nullptr;
-      v[u] = zero;
-      if (i >= total) continue;
-      const int c = int(i % cv);
-      long long r = i / cv;
-      if (dir == 0) {
-        const int sl = int(r % Sl);
-        r /= Sl;
-        const int t = int(r % Tp);
-        const int b = int(r / Tp);
-        const int col = rank * Sl + sl;
-        if (col >= S) continue;
-        const int d = t / Tl, tl = t - d * Tl;
-        if (t < T) v[u] = *reinterpret_cast<const uint4*>(local + (((size_t)b * T + t) * Sl + sl) * C + c * 8);
-        dst[u] = reinterpret_cast<uint4*>(peers.recv[d] + (((size_t)b * Tl + tl) * S + col) * C + c * 8);
-      } else {
-        const int col = int(r % Sp);
-        r /= Sp;
-        const int tl = int(r % Tl);
-        const int b = int(r / Tl);
-        const int tg = rank * Tl + tl;
-        if (tg >= T) continue;
-        const int d = col / Sl, sl = col - d * Sl;
-        if (col < S) v[u] = *reinterpret_cast<const uint4*>(local + (((size_t)b * Tl + tl) * S + col) * C + c * 8);
-        dst[u] = reinterpret_cast<uint4*>(peers.recv[d] + (((size_t)b * T + tg) * Sl + sl) * C + c * 8);
-      }
-    }
-#pragma unroll
-    for (int u = 0; u < U; ++u)
-      if (dst[u] != nullptr) *dst[u] = v[u];
-  }
-  dsp_publish(peers, rank, world, epoch);
-}
 
 // Publishes the next epoch without moving data: the producer (the proj GEMM) wrote its output into this rank's own
 // window and the consumers PULL their rows (vsb_gate_residual_dsp).
@@ -162,30 +51,6 @@ int dsp_fill_peers(DspPeers* peers, void* const* host_peer_recv, void* const* ho
 }  // namespace vsb
 
 using namespace vsb;
-
-extern "C" int vsb_dsp_scatter(const vsb_bf16* local, void* const* host_peer_recv, void* const* host_peer_flags,
-                               int rank, int world, int to_spatial_shard, int B, int T, int S, int C, unsigned epoch,
-                               void* stream) {
-  if (!local || !host_peer_recv || !host_peer_flags || world < 1 || rank < 0 || rank >= world || B <= 0 || T <= 0 ||
-      S <= 0 || C <= 0)
-    return fail(VSB_ERR_INVALID, "dsp_scatter: bad args");
-  if (world > kMaxWorld || C % 8 || !aligned16(local)) return fail(VSB_ERR_UNSUPPORTED, "dsp_scatter: world <= 16, C %% 8 == 0");
-  {
-    const long long Tp = ((T + world - 1) / world) * (long long)world, Sp = ((S + world - 1) / world) * (long long)world;
-    if ((long long)B * Tp * Sp >= (1ll << 31)) return fail(VSB_ERR_UNSUPPORTED, "dsp_scatter: too many rows");
-  }
-  DspPeers peers;
-  int rc = dsp_fill_peers(&peers, host_peer_recv, host_peer_flags, world, "dsp_scatter");
-  if (rc) return rc;
-  const int grid = num_sms() * 4;
-  if (g_opt_dsp_rowwise)
-    dsp_scatter_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const bf16*)local, peers, rank, world, to_spatial_shard,
-                                                                B, T, S, C, epoch);
-  else
-    dsp_scatter_vec_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const bf16*)local, peers, rank, world,
-                                                                    to_spatial_shard, B, T, S, C, epoch);
-  return check_launch("dsp_scatter");
-}
 
 extern "C" int vsb_dsp_signal(void* const* host_peer_flags, int rank, int world, unsigned epoch, void* stream) {
   if (!host_peer_flags || world < 1 || world > kMaxWorld || rank < 0 || rank >= world)

@@ -46,8 +46,8 @@ struct LnDspArgs {
   unsigned epoch;
 };
 
-// kMinBlocks: 3 = 80 registers, 24 resident warps per SM (one 2.3 KB row in flight each); 4 = capped at 64 registers
-// (~100 bytes of spills) for 32 resident warps: option "ln_occupancy" picks.
+// kMinBlocks: resident 256-thread blocks per SM the register budget is sized for; 3 at hidden <= 1280 = 80 registers,
+// 24 resident warps per SM (one 2.3 KB row in flight each).
 template <int kMaxVec, bool kDsp, int kMinBlocks>
 __global__ void __launch_bounds__(256, kMinBlocks) ln_modulate_kernel(const bf16* __restrict__ x, bf16* __restrict__ out,
                                                           const bf16* __restrict__ mod,
@@ -496,7 +496,7 @@ static int ln_modulate_launch(const vsb_bf16* x, vsb_bf16* out, const vsb_bf16* 
   if (dsp) {
     if (C <= 1280) VSB_LN_LAUNCH(5, true, 3, *dsp); else VSB_LN_LAUNCH(8, true, 2, *dsp);
   } else if (C <= 1280) {
-    if (g_opt_ln_occupancy >= 4) VSB_LN_LAUNCH(5, false, 4, none); else VSB_LN_LAUNCH(5, false, 3, none);
+    VSB_LN_LAUNCH(5, false, 3, none);
   } else if (C <= 2048) {
     VSB_LN_LAUNCH(8, false, 2, none);
   } else if (C <= 2304) {  // hidden 2304 (Open-Sora-Plan v1.2.0: 24 heads x 96)

@@ -13,8 +13,6 @@
 namespace vsbs {
 extern thread_local char g_err[512];
 extern std::atomic<unsigned long long> g_launches;
-// run-time kernel selection knobs (vsb_set_option)
-extern int g_opt_dsp_rowwise, g_opt_ln_occupancy;
 
 inline int fail(int code, const char* fmt, ...) {
   va_list ap;

@@ -160,6 +160,7 @@ class _Rope(nn.Module):
 
 class STDiT3(nn.Module):
     config_class = STDiT3Config
+    _fuse_dsp = True  # the P2P switch is always fused into its kernels; bench.py's dsp_parity record reads it as a label
 
     def __init__(self, config: STDiT3Config):
         super().__init__()
@@ -193,9 +194,6 @@ class STDiT3(nn.Module):
         self._text_cache = None  # per (y, mask): caption MLP output, key layout, per-block kv_linear outputs
         self._hw_cache = None
         self._final_pad = None
-        # DSP switch fused into its producer / consumer (ln_modulate stores to the peers, gate+residual pulls from
-        # them); VSB_DSP_FUSED=0 selects the standalone scatter kernel (vsb_dsp_scatter)
-        self._fuse_dsp = os.environ.get("VSB_DSP_FUSED", "1") == "1"
 
     # ------------------------------------------------------------------------------------------------------
     def initialize_weights(self):
@@ -345,10 +343,9 @@ class STDiT3(nn.Module):
 
     # ---- one block on the kernels ----------------------------------------------------------------------------
     def _switch(self, x4: torch.Tensor, T: int, S: int, to_spatial_shard: bool) -> torch.Tensor:
-        """DSP dimension switch of a [B, t, s, C] tensor (global extents T, S)."""
+        """DSP dimension switch of a [B, t, s, C] tensor (global extents T, S) over all_to_all_single, for process groups
+        without CUDA IPC; the P2P path fuses the switch into its kernels (_run_block)."""
         pm = self.parallel_manager
-        if self._dsp is not None:
-            return self._dsp.switch(x4.contiguous(), T, S, to_spatial_shard)
         if to_spatial_shard:
             out = comm.all_to_all_with_pad(x4, pm.sp_group, scatter_dim=2, gather_dim=1,
                                            scatter_pad=comm.get_pad("spatial"), gather_pad=comm.get_pad("temporal"))
@@ -367,7 +364,7 @@ class STDiT3(nn.Module):
         mod = K.modulation_table(blk.scale_shift_table, t_mlp, t0_mlp)
         pab_on = pab_mgr.enable_pab()
         reuse_attn, reuse_cross = plan
-        fused_dsp = self._dsp is not None and self._fuse_dsp and not blk.temporal and sp > 1
+        fused_dsp = self._dsp is not None and not blk.temporal and sp > 1
 
         # ---- self attention ----
         if reuse_attn:
@@ -387,21 +384,16 @@ class STDiT3(nn.Module):
             else:
                 Ba = B
                 if fused_dsp:
-                    # the modulate kernel's stores ARE the S-shard -> T-shard switch (peer stores over NVLink)
+                    # the modulate kernel's stores ARE the S-shard -> T-shard switch (peer stores over NVLink).  It
+                    # scatters the B*T (batch, frame) sequences, not the T frames of each sample: spatial attention is
+                    # independent per (b, t), and 2*20 = 40 sequences split 8 ways exactly where T = 20 would pad to 24
+                    # and leave rank 7 computing only padding (SURVEY.md section 7 "T=20 on 8 GPUs").
                     xm = self._dsp.ln_modulate_push(x, mod, mask_u8, 0, 1, B, T, S, Sg)
                     Ba, Ta, Sa = 1, xm.shape[1], xm.shape[2]
                     xm = xm.reshape(1, Ta * Sa, C)
                 elif sp > 1:  # S-sharded -> T-sharded: attention needs every patch of a frame
                     xm = K.ln_modulate(x, mod, mask_u8, 0, 1, B, T, S)
-                    if self._dsp is not None:
-                        # P2P path: scatter the B*T (batch, frame) sequences, not the T frames of each sample.
-                        # Spatial attention is independent per (b, t), so the result is identical, and 2*20 = 40
-                        # sequences split 8 ways exactly (5 each) where T = 20 would pad to 24 and leave rank 7
-                        # computing only padding (SURVEY.md section 7 "T=20 on 8 GPUs").
-                        xm = self._switch(xm.view(1, B * T, S, C), B * Tg, Sg, to_spatial_shard=False)
-                        Ba = 1
-                    else:
-                        xm = self._switch(xm.view(B, T, S, C), Tg, Sg, to_spatial_shard=False)
+                    xm = self._switch(xm.view(B, T, S, C), Tg, Sg, to_spatial_shard=False)
                     Ta, Sa = xm.shape[1], xm.shape[2]
                     xm = xm.reshape(Ba, Ta * Sa, C)
                 else:
@@ -425,10 +417,7 @@ class STDiT3(nn.Module):
             else:
                 y = K.gemm_bias_act(o.view(-1, C), a.proj.weight, a.proj.bias)
                 if not blk.temporal and sp > 1:
-                    if self._dsp is not None:
-                        y = self._switch(y.view(1, Ta, Sa, C), B * Tg, Sg, to_spatial_shard=True)
-                    else:
-                        y = self._switch(y.view(B, Ta, Sa, C), Tg, Sg, to_spatial_shard=True)
+                    y = self._switch(y.view(B, Ta, Sa, C), Tg, Sg, to_spatial_shard=True)
                 K.gate_residual(x, y.reshape(x.shape), mod, mask_u8, 2, B, T, S, out=x, cache_out=cache)
 
         # ---- cross attention ----
