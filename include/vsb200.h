@@ -135,7 +135,9 @@ int vsb_attn_short(const vsb_bf16* qkv, vsb_bf16* out, const vsb_bf16* wq, const
 /* ---- GEMM on wgmma: out[M,N] = act(A[M,K] @ W[N,K]^T + bias[N]) ---------------------------------------------
  * replaces every nn.Linear on the path (attentions.py:59,107,156-157; timm Mlp fc1/fc2) and the tanh-GELU between
  * fc1 and fc2 (models/modules/activations.py:3).  bf16 in, fp32 accumulate in registers, bf16 out.
- *   act: 0 = none, 1 = gelu_tanh applied to bf16(acc+bias) (the eager rounding point).
+ *   act: 0 = none, 1 = gelu_tanh applied to bf16(acc+bias) (the eager rounding point), 2 = exact (erf) GELU applied to
+ *   bf16(acc+bias): F.gelu after project_in of Open-Sora-Plan v1.2.0's FeedForward_Conv2d
+ *   (models/transformers/open_sora_plan_v120_transformer_3d.py:1080-1082).
  *   Requirements: K % 8 == 0, N % 8 == 0, 16-byte aligned pointers, row-major contiguous. */
 int vsb_gemm_bias_act(const vsb_bf16* A, const vsb_bf16* W, const vsb_bf16* bias, vsb_bf16* out, int M, int N, int K,
                       int act, void* stream);
@@ -166,6 +168,29 @@ int vsb_attn_flash_strided(const vsb_bf16* q, const vsb_bf16* k, const vsb_bf16*
                            int H, int D, long long q_row_stride, long long q_batch_stride, long long kv_row_stride,
                            long long kv_batch_stride, long long out_row_stride, long long out_batch_stride,
                            const int* host_kv_lens, float scale, void* stream);
+
+/* ---- Open-Sora-Plan v1.2.0 conv down-sampler variants (downsampler = "k333_s222" / "k33_s22") ------------------------
+ * Depth-wise attention down-sampler: replaces DownSampler3d / DownSampler2d.forward
+ * (models/transformers/open_sora_plan_v120_transformer_3d.py:735-834, called at :872-874): rearrange to NCDHW, depth-wise
+ * Conv3d / Conv2d (zero "same" padding, bias) + shortcut, rearrange into dt*dh*dw interleaved sub-grids.
+ *   x      [B, T*H*W, C] token-major;  w_taps [kt*kh*kw, C] (conv.weight [C, 1, kt, kh, kw] transposed tap-major);  bias [C]
+ *   out    [(B dt dh dw), (T/dt H/dh W/dw), C]: token (b, t, h, w) lands in sub-grid ((b*dt + t%dt)*dh + h%dh)*dw + w%dw
+ *          at position ((t/dt)*(H/dh) + h/dh)*(W/dw) + w/dw.  Rounds as torch's eager GPU chain: bf16(conv), + bias,
+ *          + x, each rounded to 16 bits.
+ *   kt in {1, 3}, kh and kw in {3, 5}; dt, dh, dw divide T, H, W.  Otherwise VSB_ERR_UNSUPPORTED / VSB_ERR_INVALID. */
+int vsb_dwconv_shuffle(const vsb_bf16* x, const vsb_bf16* w_taps, const vsb_bf16* bias, vsb_bf16* out, int B, int T, int H,
+                       int W, int C, int kt, int kh, int kw, int dt, int dh, int dw, void* stream);
+/* DownSampler.reverse (:787-790, :829-833, applied at :959-960) fused into the gate + residual of the attention branch:
+ *   out[b, (t h w)] = bf16(x + bf16(gate * y[sub-grid row of (b, t, h, w)])), gate = mod[0, b, gate_row, :];
+ *   x, out [B, T*H*W, C] (out may alias x); y [(B dt dh dw), (T/dt H/dh W/dw), C] as vsb_dwconv_shuffle lays it out. */
+int vsb_gate_residual_unshuffle(const vsb_bf16* x, const vsb_bf16* y, vsb_bf16* out, const vsb_bf16* mod, int gate_row, int B,
+                                int T, int H, int W, int C, int dt, int dh, int dw, void* stream);
+/* Depth-wise part of FeedForward_Conv2d (:1033-1088): per frame, out = h + dw5x5(h) + dw3x3(h) + dw1x1(h) with the eager
+ * rounding bf16(bf16(bf16(h + c5) + c3) + c1), ck = bf16(bf16(conv_k(h)) + bias_k), zero "same" padding.
+ *   h, out [BT, H, W, C] token-major (C = the 2 x hidden width);  w_taps [25 + 9 + 1, C]: the 5x5 taps, then the 3x3
+ *   taps, then the 1x1 tap, each tap-major;  bias [3, C] (5x5, 3x3, 1x1). */
+int vsb_dwconv_ffn(const vsb_bf16* h, const vsb_bf16* w_taps, const vsb_bf16* bias, vsb_bf16* out, int BT, int H, int W, int C,
+                   void* stream);
 
 /* ---- Pyramid Attention Broadcast gate (host integer logic, bit-exact) -------------------------------------------
  * replaces PABManager.if_broadcast_{spatial,temporal,cross}: core/pab/pab_mgr.py:54-91.
@@ -255,6 +280,12 @@ int vsb_attn_flash_strided_f16(const vsb_f16* q, const vsb_f16* k, const vsb_f16
                            int H, int D, long long q_row_stride, long long q_batch_stride, long long kv_row_stride,
                            long long kv_batch_stride, long long out_row_stride, long long out_batch_stride,
                            const int* host_kv_lens, float scale, void* stream);
+int vsb_dwconv_shuffle_f16(const vsb_f16* x, const vsb_f16* w_taps, const vsb_f16* bias, vsb_f16* out, int B, int T, int H,
+                           int W, int C, int kt, int kh, int kw, int dt, int dh, int dw, void* stream);
+int vsb_gate_residual_unshuffle_f16(const vsb_f16* x, const vsb_f16* y, vsb_f16* out, const vsb_f16* mod, int gate_row, int B,
+                                    int T, int H, int W, int C, int dt, int dh, int dw, void* stream);
+int vsb_dwconv_ffn_f16(const vsb_f16* h, const vsb_f16* w_taps, const vsb_f16* bias, vsb_f16* out, int BT, int H, int W, int C,
+                       void* stream);
 
 #ifdef __cplusplus
 }

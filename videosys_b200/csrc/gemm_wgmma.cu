@@ -42,6 +42,9 @@ __device__ __forceinline__ float gelu_tanh_f(float x) {
   return x * r;
 }
 
+// exact GELU (F.gelu, approximate='none') as torch's CUDA kernel evaluates it: x * 0.5 * (1 + erf(x / sqrt(2))) in fp32
+__device__ __forceinline__ float gelu_erf_f(float x) { return x * 0.5f * (1.f + erff(x * 0.70710678118654752440f)); }
+
 // ACT == 2: out = resid + g, g = bf16(gate * y) (gate_row >= 0, per-frame t/t0 select) or g = y (plain residual add),
 // y = bf16(acc + bias): the eager chain of open_sora_transformer_3d.py (Linear, gate multiply, residual add) in the epilogue.
 struct EpiArgs {
@@ -156,6 +159,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
         x0 = gelu_tanh_f(rbf(x0));
         x1 = gelu_tanh_f(rbf(x1));
       }
+      if (ACT == 3) {
+        x0 = gelu_erf_f(rbf(x0));
+        x1 = gelu_erf_f(rbf(x1));
+      }
       if (ACT == 2) {
         const long long grow = (long long)m0 + row;
         if (grow < M && gcol < N) {
@@ -202,7 +209,7 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tw, const CUten
   return check_launch("gemm_wgmma");
 }
 
-// act: 0 none, 1 tanh-GELU, 2 fused residual (ep->resid != nullptr)
+// act: 0 none, 1 tanh-GELU, 2 fused residual (ep->resid != nullptr), 3 erf-GELU
 static int gemm_dispatch(const void* A, const void* W, const void* bias, void* out, int M, int N, int K, int act,
                          cudaStream_t st, const EpiArgs& ep) {
   // tile width: 192 divides every STDiT3 / CogVideoX / Latte width (1152, 1920, 2304, 3072, 3456, 4608, 7680); narrow
@@ -226,6 +233,7 @@ static int gemm_dispatch(const void* A, const void* W, const void* bias, void* o
   const bf16* b = (const bf16*)bias;
 #define VSB_GEMM_CASE(bn)                                                     \
   if (BN == bn) {                                                             \
+    if (act == 3) return launch_gemm<bn, 3>(ta, tw, tc, b, M, N, K, st, ep);  \
     if (act == 2) return launch_gemm<bn, 2>(ta, tw, tc, b, M, N, K, st, ep);  \
     if (act == 1) return launch_gemm<bn, 1>(ta, tw, tc, b, M, N, K, st, ep);  \
     return launch_gemm<bn, 0>(ta, tw, tc, b, M, N, K, st, ep);                \
@@ -245,8 +253,9 @@ extern "C" int VSB_API(vsb_gemm_bias_act)(const vsb_bf16* A, const vsb_bf16* W, 
   if (!A || !W || !out || M <= 0 || N <= 0 || K <= 0) return fail(VSB_ERR_INVALID, "gemm: bad args");
   if (K % 8 || N % 8 || !aligned16(A) || !aligned16(W) || !aligned16(out))
     return fail(VSB_ERR_UNSUPPORTED, "gemm: need K %% 8 == 0, N %% 8 == 0, 16B-aligned pointers (M=%d N=%d K=%d)", M, N, K);
-  if (act != 0 && act != 1) return fail(VSB_ERR_INVALID, "gemm: act=%d", act);
-  return gemm_dispatch(A, W, bias, out, M, N, K, act, (cudaStream_t)stream, EpiArgs{nullptr, nullptr, nullptr, -1, 1, 1, 1});
+  if (act < 0 || act > 2) return fail(VSB_ERR_INVALID, "gemm: act=%d", act);
+  // public act 2 (erf-GELU) is epilogue 3: epilogue 2 is the fused residual of vsb_gemm_bias_residual
+  return gemm_dispatch(A, W, bias, out, M, N, K, act == 2 ? 3 : act, (cudaStream_t)stream, EpiArgs{nullptr, nullptr, nullptr, -1, 1, 1, 1});
 }
 
 // Fused epilogue: out = resid + [gate *] (A @ W^T + bias), see include/vsb200.h.

@@ -202,6 +202,45 @@ def residual_add(x, y, out=None):
     return out
 
 
+def dwconv_shuffle(x, w_taps, bias, B, T, H, W, ksize, down):
+    """Depth-wise conv (kernel ksize = (kt, kh, kw), zero "same" padding) + bias + shortcut of x [B, T*H*W, C], stored in
+    the sub-grid order [(B dt dh dw), (T/dt H/dh W/dw), C] of down = (dt, dh, dw); w_taps [kt*kh*kw, C] tap-major."""
+    lib, st = _prep(x, w_taps, bias)
+    _bf16(x, "x")
+    _same_dtype(x, w_taps, bias)
+    Cc = x.shape[-1]
+    dt, dh, dw = down
+    out = torch.empty(B * dt * dh * dw, (T // dt) * (H // dh) * (W // dw), Cc, dtype=x.dtype, device=x.device)
+    with _Timed("dwconv_shuffle", 2 * x.numel() * 2):
+        _lib.check(_fn(lib, "vsb_dwconv_shuffle", x)(_p(x), _p(w_taps), _p(bias), _p(out), B, T, H, W, Cc, *ksize, dt, dh, dw, st),
+                   "dwconv_shuffle")
+    return out
+
+
+def gate_residual_unshuffle(x, y, mod, gate_row, B, T, H, W, down, out=None):
+    """out = x + gate * y with y in the sub-grid order of dwconv_shuffle (read through the inverse regrouping)."""
+    lib, st = _prep(x, y, mod, out)
+    _same_dtype(x, y, mod, out)
+    Cc = x.shape[-1]
+    out = torch.empty_like(x) if out is None else out
+    with _Timed("gate_residual", 3 * x.numel() * 2):
+        _lib.check(_fn(lib, "vsb_gate_residual_unshuffle", x)(_p(x), _p(y), _p(out), _p(mod), gate_row, B, T, H, W, Cc, *down, st),
+                   "gate_residual_unshuffle")
+    return out
+
+
+def dwconv_ffn(h, w_taps, bias, BT, H, W):
+    """h + dw5x5(h) + dw3x3(h) + dw1x1(h) per frame of h [BT, H, W, C] (token-major); w_taps [35, C], bias [3, C]."""
+    lib, st = _prep(h, w_taps, bias)
+    _bf16(h, "h")
+    _same_dtype(h, w_taps, bias)
+    Cc = h.shape[-1]
+    out = torch.empty_like(h)
+    with _Timed("dwconv_ffn", 2 * h.numel() * 2):
+        _lib.check(_fn(lib, "vsb_dwconv_ffn", h)(_p(h), _p(w_taps), _p(bias), _p(out), BT, H, W, Cc, st), "dwconv_ffn")
+    return out
+
+
 def qk_rmsnorm_(qkv, wq, wk, H, D, eps=1e-6, rope_cos=None, rope_sin=None, pos_div=1, pos_mod=1):
     """In-place per-head RMSNorm of q and k; with rope tables also RoPE at position (row // pos_div) % pos_mod."""
     lib, st = _prep(qkv, wq, wk, rope_cos, rope_sin)
