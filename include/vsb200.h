@@ -192,6 +192,21 @@ int vsb_gate_residual_unshuffle(const vsb_bf16* x, const vsb_bf16* y, vsb_bf16* 
 int vsb_dwconv_ffn(const vsb_bf16* h, const vsb_bf16* w_taps, const vsb_bf16* bias, vsb_bf16* out, int BT, int H, int W, int C,
                    void* stream);
 
+/* ---- Open-Sora-Plan v1.1.0 KV compression (compress_kv_factor = k > 1, second-half blocks) ----------------------------
+ * replaces Attention.sr + Attention.norm and the rearranges around them in AttnProcessor2_0.__call__
+ * (models/transformers/open_sora_plan_v110_transformer_3d.py:1181-1197; layers built by _init_compress :1101-1122):
+ * depth-wise Conv2d / Conv1d with stride = kernel (floors), + bias, then nn.LayerNorm(C) (affine).
+ *   x     [B, T, H, W, C] token-major;  window (kt, kh, kw): spatial (1, k, k) per frame, temporal (k, 1, 1) per patch;
+ *   pad_t leading copies of frame 0 (the reference prepends k - 1 of them when T is odd, :1190-1192);
+ *   w_taps [kt*kh*kw, C] (sr.weight transposed tap-major);  bias, ln_w, ln_b [C];  eps = norm.eps (1e-5);
+ *   out   [B, (T+pad_t)/kt, H/kh, W/kw, C] token-major (the layout of the queries).
+ *   round_conv = 1: bf16(bf16(conv) + bias), what cuDNN gives for the spatial Conv2d on the reference's channels-last view;
+ *   round_conv = 0: bf16(bias + conv) rounded once, ATen's native depthwise kernel, which the Conv1d takes.
+ *   The LayerNorm rounds once at its output.  VSB_ERR_INVALID for an empty output grid or C % 8 != 0; C <= 3072. */
+int vsb_kv_compress(const vsb_bf16* x, const vsb_bf16* w_taps, const vsb_bf16* bias, const vsb_bf16* ln_w, const vsb_bf16* ln_b,
+                    vsb_bf16* out, int B, int T, int H, int W, int C, int kt, int kh, int kw, int pad_t, float eps, int round_conv,
+                    void* stream);
+
 /* ---- Pyramid Attention Broadcast gate (host integer logic, bit-exact) -------------------------------------------
  * replaces PABManager.if_broadcast_{spatial,temporal,cross}: core/pab/pab_mgr.py:54-91.
  * Returns 1 (reuse the cached tensor) or 0; *count advances on every call and wraps modulo steps.
@@ -286,6 +301,9 @@ int vsb_gate_residual_unshuffle_f16(const vsb_f16* x, const vsb_f16* y, vsb_f16*
                                     int T, int H, int W, int C, int dt, int dh, int dw, void* stream);
 int vsb_dwconv_ffn_f16(const vsb_f16* h, const vsb_f16* w_taps, const vsb_f16* bias, vsb_f16* out, int BT, int H, int W, int C,
                        void* stream);
+int vsb_kv_compress_f16(const vsb_f16* x, const vsb_f16* w_taps, const vsb_f16* bias, const vsb_f16* ln_w, const vsb_f16* ln_b,
+                        vsb_f16* out, int B, int T, int H, int W, int C, int kt, int kh, int kw, int pad_t, float eps,
+                        int round_conv, void* stream);
 
 #ifdef __cplusplus
 }

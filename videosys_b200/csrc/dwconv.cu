@@ -9,6 +9,9 @@
 // rows its neighbours in the block read too, so they come from L1; zero "same" padding = out-of-range taps load zeros.
 // Depth-wise weights arrive tap-major ([taps, C]: one 16-byte load per tap gives 8 channels).  fp32 accumulation, 16-bit
 // rounding at the points where the reference's eager ops round.
+//
+// Also Open-Sora-Plan v1.1.0's KV compression (compress_kv_factor): the strided depth-wise conv + LayerNorm that makes the
+// keys / values of its second-half blocks (kv_compress_kernel, one warp per output row; see its comment).
 #include "vsb_common.cuh"
 #include "vsb_host.h"
 
@@ -221,6 +224,133 @@ __global__ void __launch_bounds__(256) gate_residual_unshuffle_kernel(const bf16
   }
 }
 
+__device__ __forceinline__ float kvc_warp_sum(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// KV compression of Open-Sora-Plan v1.1.0 (attn.sr + attn.norm): x [B, T, H, W, C] token-major, window (kt, kh, kw) with
+// stride = window, pad_t leading copies of frame 0; out [B, (T+pad_t)/kt, H/kh, W/kw, C] token-major.  One warp per output
+// row, the row in registers (lane owns vectors lane, lane+32, ...).  Conv rounding (round_conv):
+//   1: bf16(bf16(conv) + bias) -- cuDNN, which torch picks for the spatial Conv2d because the reference hands it a
+//      channels-last view of the tokens (it rounds the conv, then adds the bias as a separate 16-bit op);
+//   0: bf16(bias + conv), bias first in the fp32 sum -- ATen's native depthwise kernel, which the Conv1d takes (conv1d
+//      makes its input contiguous).
+// Then LayerNorm (two-pass fp32 statistics, affine) rounded once.
+template <int kMaxVec>
+__global__ void __launch_bounds__(256) kv_compress_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w,
+                                                          const bf16* __restrict__ bias, const bf16* __restrict__ ln_w,
+                                                          const bf16* __restrict__ ln_b, bf16* __restrict__ out, int T,
+                                                          int H, int W, int C, int kt, int kh, int kw, int pad_t, int Tc,
+                                                          int Hc, int Wc, float eps, int round_conv, long long rows) {
+  const int lane = threadIdx.x & 31;
+  const int nvec = C >> 3;
+  const int taps = kt * kh * kw;
+  const long long stride = (long long)gridDim.x * (blockDim.x >> 5);
+  for (long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); row < rows; row += stride) {
+    long long r = row;
+    const int wc = int(r % Wc);
+    r /= Wc;
+    const int hc = int(r % Hc);
+    r /= Hc;
+    const int tc = int(r % Tc);
+    const int b = int(r / Tc);
+    float acc[kMaxVec][8];
+#pragma unroll
+    for (int i = 0; i < kMaxVec; ++i) {
+      const int vi = lane + i * 32;
+      if (vi < nvec && !round_conv) {
+        V8 bv;
+        bv.u = __ldg(reinterpret_cast<const uint4*>(bias + vi * 8));
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const float2 f = e2_to_float2(bv.h[j]);
+          acc[i][2 * j] = f.x;
+          acc[i][2 * j + 1] = f.y;
+        }
+      } else {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) acc[i][j] = 0.f;
+      }
+    }
+    // taps in (it, ih, iw) order: the order of the weight's [kt, kh, kw] extent and of ATen's native accumulation
+#pragma unroll 1
+    for (int tap = 0; tap < taps; ++tap) {
+      const int iw = tap % kw, ih = (tap / kw) % kh, it = tap / (kw * kh);
+      const int tp = tc * kt + it - pad_t;
+      const int t = tp < 0 ? 0 : tp;
+      const bf16* xr = x + ((((size_t)b * T + t) * H + hc * kh + ih) * W + wc * kw + iw) * C;
+      const bf16* wr = w + (size_t)tap * C;
+      V8 xv[kMaxVec];
+#pragma unroll
+      for (int i = 0; i < kMaxVec; ++i) {
+        const int vi = lane + i * 32;
+        if (vi < nvec) xv[i].u = __ldg(reinterpret_cast<const uint4*>(xr + vi * 8));
+      }
+#pragma unroll
+      for (int i = 0; i < kMaxVec; ++i) {
+        const int vi = lane + i * 32;
+        if (vi < nvec) {
+          V8 wv;
+          wv.u = __ldg(reinterpret_cast<const uint4*>(wr + vi * 8));
+          fma8(acc[i], xv[i], wv);
+        }
+      }
+    }
+    float sum = 0.f;
+#pragma unroll
+    for (int i = 0; i < kMaxVec; ++i) {
+      const int vi = lane + i * 32;
+      if (vi < nvec) {
+        V8 bv;
+        if (round_conv) bv.u = __ldg(reinterpret_cast<const uint4*>(bias + vi * 8));
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          float y0 = rbf(acc[i][2 * j]), y1 = rbf(acc[i][2 * j + 1]);
+          if (round_conv) {
+            const float2 f = e2_to_float2(bv.h[j]);
+            y0 = rbf(y0 + f.x);
+            y1 = rbf(y1 + f.y);
+          }
+          acc[i][2 * j] = y0;
+          acc[i][2 * j + 1] = y1;
+          sum += y0 + y1;
+        }
+      }
+    }
+    const float mean = kvc_warp_sum(sum) / (float)C;
+    float sq = 0.f;
+#pragma unroll
+    for (int i = 0; i < kMaxVec; ++i) {
+      if (lane + i * 32 < nvec) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float d = acc[i][j] - mean;
+          sq += d * d;
+        }
+      }
+    }
+    const float rstd = rsqrtf(kvc_warp_sum(sq) / (float)C + eps);
+    bf16* orow = out + (size_t)row * C;
+#pragma unroll
+    for (int i = 0; i < kMaxVec; ++i) {
+      const int vi = lane + i * 32;
+      if (vi < nvec) {
+        V8 gv, bv, o;
+        gv.u = __ldg(reinterpret_cast<const uint4*>(ln_w + vi * 8));
+        bv.u = __ldg(reinterpret_cast<const uint4*>(ln_b + vi * 8));
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const float2 g = e2_to_float2(gv.h[j]), bb = e2_to_float2(bv.h[j]);
+          o.h[j] = floats_to_e2((acc[i][2 * j] - mean) * rstd * g.x + bb.x, (acc[i][2 * j + 1] - mean) * rstd * g.y + bb.y);
+        }
+        *reinterpret_cast<uint4*>(orow + vi * 8) = o.u;
+      }
+    }
+  }
+}
+
 }  // namespace vsb
 
 using namespace vsb;
@@ -292,4 +422,34 @@ extern "C" int VSB_API(vsb_gate_residual_unshuffle)(const vsb_bf16* x, const vsb
   gate_residual_unshuffle_kernel<<<(int)(blocks < cap ? blocks : cap), 256, 0, (cudaStream_t)stream>>>(
       (const bf16*)x, (const bf16*)y, (bf16*)out, (const bf16*)mod, gate_row, T, H, W, C, dt, dh, dw, nvec);
   return check_launch("gate_residual_unshuffle");
+}
+
+extern "C" int VSB_API(vsb_kv_compress)(const vsb_bf16* x, const vsb_bf16* w_taps, const vsb_bf16* bias, const vsb_bf16* ln_w,
+                                        const vsb_bf16* ln_b, vsb_bf16* out, int B, int T, int H, int W, int C, int kt, int kh,
+                                        int kw, int pad_t, float eps, int round_conv, void* stream) {
+  if (B <= 0 || T <= 0 || H <= 0 || W <= 0 || C <= 0 || kt <= 0 || kh <= 0 || kw <= 0 || pad_t < 0 ||
+      (round_conv != 0 && round_conv != 1))
+    return fail(VSB_ERR_INVALID, "kv_compress: bad args");
+  const int Tc = (T + pad_t) / kt, Hc = H / kh, Wc = W / kw;
+  if (Tc == 0 || Hc == 0 || Wc == 0)  // checked before the pointers: an empty output tensor has no storage
+    return fail(VSB_ERR_INVALID, "kv_compress: empty output grid (%d+%d frames, %dx%d) for window %dx%dx%d", T, pad_t, H, W, kt, kh, kw);
+  if (!x || !w_taps || !bias || !ln_w || !ln_b || !out) return fail(VSB_ERR_INVALID, "kv_compress: null pointer");
+  if (C % 8) return fail(VSB_ERR_INVALID, "kv_compress: C %% 8 != 0 (C=%d)", C);
+  if (C > 3072 || !aligned16(x) || !aligned16(w_taps) || !aligned16(bias) || !aligned16(ln_w) || !aligned16(ln_b) || !aligned16(out))
+    return fail(VSB_ERR_UNSUPPORTED, "kv_compress: need C <= 3072 and 16B-aligned pointers");
+  if ((long long)B * T * H * W * C >= (1ll << 40)) return fail(VSB_ERR_UNSUPPORTED, "kv_compress: too large");
+  const long long rows = (long long)B * Tc * Hc * Wc;
+  long long blocks = (rows + 7) / 8, cap = (long long)num_sms() * 16;
+  const int grid = (int)(blocks < cap ? blocks : cap);
+  cudaStream_t st = (cudaStream_t)stream;
+#define VSB_KVC(MV)                                                                                                    \
+  kv_compress_kernel<MV><<<grid, 256, 0, st>>>((const bf16*)x, (const bf16*)w_taps, (const bf16*)bias, (const bf16*)ln_w, \
+                                               (const bf16*)ln_b, (bf16*)out, T, H, W, C, kt, kh, kw, pad_t, Tc, Hc, Wc, eps, \
+                                               round_conv, rows)
+  if (C <= 1280)
+    VSB_KVC(5);
+  else
+    VSB_KVC(12);
+#undef VSB_KVC
+  return check_launch("kv_compress");
 }

@@ -241,6 +241,22 @@ def dwconv_ffn(h, w_taps, bias, BT, H, W):
     return out
 
 
+def kv_compress(x, w_taps, bias, ln_w, ln_b, B, T, H, W, window, pad_t=0, eps=1e-5, round_conv=True):
+    """LayerNorm(depth-wise conv(x) + bias) with stride = window (kt, kh, kw) over x [B, T, H, W, C] (token-major), after
+    pad_t leading copies of frame 0; returns [B, (T+pad_t)//kt, H//kh, W//kw, C].  w_taps [kt*kh*kw, C] tap-major.
+    round_conv: round the conv before the bias is added (torch's cuDNN path) instead of once after it (ATen's native one)."""
+    lib, st = _prep(x, w_taps, bias, ln_w, ln_b)
+    _bf16(x, "x")
+    _same_dtype(x, w_taps, bias, ln_w, ln_b)
+    Cc = x.shape[-1]
+    kt, kh, kw = window
+    out = torch.empty(B, (T + pad_t) // kt, H // kh, W // kw, Cc, dtype=x.dtype, device=x.device)
+    with _Timed("kv_compress", (x.numel() + out.numel()) * 2):
+        _lib.check(_fn(lib, "vsb_kv_compress", x)(_p(x), _p(w_taps), _p(bias), _p(ln_w), _p(ln_b), _p(out), B, T, H, W, Cc, kt, kh,
+                                                  kw, pad_t, eps, int(bool(round_conv)), st), "kv_compress")
+    return out
+
+
 def qk_rmsnorm_(qkv, wq, wk, H, D, eps=1e-6, rope_cos=None, rope_sin=None, pos_div=1, pos_mod=1):
     """In-place per-head RMSNorm of q and k; with rope tables also RoPE at position (row // pos_div) % pos_mod."""
     lib, st = _prep(qkv, wq, wk, rope_cos, rope_sin)

@@ -55,6 +55,22 @@ def temporal_attention(qkv, B, T, S, H, D, scale, short_max, wq=None, wk=None, r
     return o
 
 
+def temporal_cross_attention(q, kv, B, T, Tk, S, H, D, scale):
+    """Attention over frames at every (sample, patch) with fewer key frames than query frames: q [B*T*S, H*D] token-major,
+    kv [B*Tk*S, 2, H*D] (packed k | v, token-major over Tk frames).  One ``attn_flash`` per sample over strided views
+    (batch = patch, q row = frame, kv row = key frame).  Returns [B*T*S, H*D] in the order of q."""
+    if S > 65535:
+        raise RuntimeError("temporal flash attention: more than 65535 patches per frame")
+    C = H * D
+    q = q.view(B * T * S, C)
+    o = torch.empty(B * T * S, C, dtype=q.dtype, device=q.device)
+    for b in range(B):
+        kvb = kv[b * Tk * S:]
+        kernels.attn_flash(q[b * T * S:], kvb[:, 0], kvb[:, 1], S, T, Tk, H, D, S * C, C, S * 2 * C, 2 * C, scale,
+                           out=o[b * T * S:], out_row_stride=S * C, out_batch_stride=C)
+    return o
+
+
 def packed_self_attention(qkv, nb, n, H, D, scale, short_max=None, wq=None, wk=None, sdpa=False):
     """Self-attention of nb sequences of n tokens in one packed [nb*n, 3, H, D] buffer; returns [nb, n, H*D].
     n <= short_max runs ``attn_short`` (q / k norm inside the kernel); otherwise the norm pass (when wq is given) and

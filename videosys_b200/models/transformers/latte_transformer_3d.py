@@ -24,7 +24,8 @@ import torch.nn as nn
 from ... import kernels
 from ...core.distributed import comm
 from ...core.pab import pab_mgr
-from ._attention import apply_rope_, cross_attention, packed_self_attention, temporal_attention
+from ._attention import (apply_rope_, cross_attention, packed_self_attention, temporal_attention,
+                         temporal_cross_attention)
 from ._common import (AdaLNSingle, Lin2, PatchEmbed2D, ada_norm_single, ada_norm_single_out, fused_linear, parallel_manager,
                       patch_embed_frames, pos_embed_2d, sincos_1d)
 
@@ -70,6 +71,36 @@ class LatteBlock(nn.Module):
         self.last_attn = self.last_cross = None
 
 
+def _sr_taps(cache, sr):
+    """sr.weight [C, 1, *window] as [taps, C] (tap-major), kept in ``cache`` and rebuilt when the parameter changes."""
+    ver = (sr.weight.data_ptr(), sr.weight._version, sr.weight.dtype)
+    hit = cache.get("sr")
+    if hit is None or hit[0] != ver:
+        hit = cache["sr"] = (ver, sr.weight.reshape(sr.weight.shape[0], -1).t().contiguous())
+    return hit[1]
+
+
+def _compressed_attention(blk, xm, B, Fr, S, grid, pad_t, H, D):
+    """Self-attention of a block with Open-Sora-Plan v1.1.0's KV compression (open_sora_plan_v110_transformer_3d.py:1181-1197):
+    queries from every modulated token xm [B*Fr*S, C], keys / values from attn1.norm(attn1.sr(xm)) -- a stride-k depth-wise
+    conv over the (h, w) = grid patches of each frame (spatial block) or over the Fr frames of each patch after pad_t copies of
+    frame 0 (temporal block).  Returns [B*Fr*S, C] in the order of xm."""
+    a1, C = blk.attn1, H * D
+    k = a1.sr.stride[0]
+    q = kernels.gemm_bias_act(xm, a1.to_q.weight, a1.to_q.bias)
+    taps = _sr_taps(blk._fused, a1.sr)
+    if blk.temporal:  # Conv1d: ATen's native depthwise kernel (one rounding after the bias)
+        xc = kernels.kv_compress(xm, taps, a1.sr.bias, a1.norm.weight, a1.norm.bias, B, Fr, S, 1, (k, 1, 1), pad_t, a1.norm.eps,
+                                 round_conv=False)
+    else:  # Conv2d on a channels-last view: cuDNN (the conv rounded, then the bias added)
+        xc = kernels.kv_compress(xm, taps, a1.sr.bias, a1.norm.weight, a1.norm.bias, B, Fr, grid[0], grid[1], (1, k, k), 0,
+                                 a1.norm.eps, round_conv=True)
+    kv = kernels.gemm_bias_act(xc.view(-1, C), *fused_linear(blk._fused, a1.to_k, a1.to_v)).view(-1, 2, C)
+    if blk.temporal:
+        return temporal_cross_attention(q, kv, B, Fr, xc.shape[1], S, H, D, D**-0.5)
+    return cross_attention(q, kv, B * Fr, S, xc.shape[2] * xc.shape[3], H, D, D**-0.5).view(-1, C)
+
+
 class LatteBlockStack(nn.Module):
     def __init__(self, hidden_size=1152, num_heads=16, depth=28):
         super().__init__()
@@ -83,7 +114,8 @@ class LatteBlockStack(nn.Module):
 
     @torch.no_grad()
     def forward(self, x: torch.Tensor, enc: torch.Tensor, timestep6: torch.Tensor, temp_pos_embed: Optional[torch.Tensor] = None,
-                ts_int: Optional[int] = None, all_timesteps=None, sp_group=None, rope: Optional[dict] = None, enc_lens=None):
+                ts_int: Optional[int] = None, all_timesteps=None, sp_group=None, rope: Optional[dict] = None, enc_lens=None,
+                kv_grid=None, kv_pad_t: int = 0):
         """x [B, F, S, C] fp16 / bf16 (CUDA), enc [B, L, C], timestep6 [B, 6C]; returns [B, F, S, C].
         PAB (reference blocks :372-517, :700-824): ts_int = int(org_timestep[0]) on the host, all_timesteps = the
         scheduler's timestep list (python ints) for the MLP skip windows.
@@ -92,7 +124,9 @@ class LatteBlockStack(nn.Module):
         the attention (qkv, softmax, out projection) and switches the result back (pads: comm.get_pad).
         rope (Open-Sora-Plan v1.1.0, open_sora_plan_v110_transformer_3d.py:1217-1232): {"spatial": (cos, sin_signed, half),
         "temporal": (...)} tables of ``vsb_qk_rope_halves`` indexed by the token's patch / frame; enc_lens: valid text tokens per
-        sample (the reference's -10000 bias on padded keys, :2440-2444)."""
+        sample (the reference's -10000 bias on padded keys, :2440-2444).
+        kv_grid / kv_pad_t (Open-Sora-Plan v1.1.0 KV compression, blocks whose attn1 has ``sr``): the (h, w) patch grid of a
+        frame and the leading copies of frame 0 the temporal compression reads."""
         K = kernels
         K.require_cuda(x, "Latte / Open-Sora-Plan blocks", half_only=True)
         B, Fr, S, C = x.shape
@@ -128,14 +162,17 @@ class LatteBlockStack(nn.Module):
                         Ft, St = xm.shape[1], xm.shape[2]
                         xm = xm.view(B * Ft * St, C)
                     a1 = blk.attn1
-                    qkv = K.gemm_bias_act(xm, *fused_linear(blk._fused, a1.to_q, a1.to_k, a1.to_v))
-                    if blk.temporal:
-                        o = temporal_attention(qkv, B, Ft, St, H, D, D**-0.5, 32, sdpa=True,
-                                               rope=None if rope is None else rope["temporal"])
+                    if hasattr(a1, "sr"):  # Open-Sora-Plan v1.1.0 KV compression (only its second-half blocks have sr)
+                        o = _compressed_attention(blk, xm, B, Ft, St, kv_grid, kv_pad_t, H, D)
                     else:
-                        if rope is not None:
-                            apply_rope_(qkv, rope["spatial"], H, D, pos_div=1, pos_mod=S)
-                        o = packed_self_attention(qkv, B * Fr, S, H, D, D**-0.5, short_max=29, sdpa=True)
+                        qkv = K.gemm_bias_act(xm, *fused_linear(blk._fused, a1.to_q, a1.to_k, a1.to_v))
+                        if blk.temporal:
+                            o = temporal_attention(qkv, B, Ft, St, H, D, D**-0.5, 32, sdpa=True,
+                                                   rope=None if rope is None else rope["temporal"])
+                        else:
+                            if rope is not None:
+                                apply_rope_(qkv, rope["spatial"], H, D, pos_div=1, pos_mod=S)
+                            o = packed_self_attention(qkv, B * Fr, S, H, D, D**-0.5, short_max=29, sdpa=True)
                     y = K.gemm_bias_act(o.view(-1, C), blk.attn1.to_out[0].weight, blk.attn1.to_out[0].bias)
                     if switch:  # patch shard -> frame shard (scatter F, gather S)
                         y = comm.all_to_all_with_pad(y.view(B, Ft, St, C), sp_group, scatter_dim=1, gather_dim=2,

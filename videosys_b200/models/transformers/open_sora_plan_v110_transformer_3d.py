@@ -12,10 +12,16 @@ of this package) with two additions that exist only here:
     (each half of the head for one axis), 1-D over the frame index in the temporal blocks, linear position scaling with its
     integer truncation (:187-196, :244-252); ``vsb_qk_rope_halves`` in place on the packed qkv, tables built exactly as the
     reference builds its 16-bit cos / sin (angles rounded to the compute dtype before the cos: :149-152);
-  * the text padding mask (:2440-2444, a -10000 bias on padded keys) as per-sample key counts of ``vsb_attn_flash``.
+  * the text padding mask (:2440-2444, a -10000 bias on padded keys) as per-sample key counts of ``vsb_attn_flash``;
+  * KV compression (``compress_kv_factor`` = k > 1, only without RoPE: :2200): the second-half blocks (d >= num_layers // 2,
+    :2283-2320) carry ``attn1.sr`` (depth-wise Conv2d k x k / Conv1d k, stride k) and ``attn1.norm`` (LayerNorm, eps 1e-5);
+    their keys and values come from norm(sr(tokens)) over the patch grid of each frame (spatial) or the frames of each patch
+    after k - 1 copies of frame 0 when the frame count is odd (temporal), :1181-1197 -- ``vsb_kv_compress``, then the
+    k | v GEMM on the compressed rows and ``vsb_attn_flash`` with fewer keys than queries.  The compressed latent mask
+    (:2497) is all ones, as every mask this front end accepts.
 
-State-dict compatible with the reference / HF ``LanguageBind/Open-Sora-Plan-v1.1.0`` transformer.  Not built: KV
-compression (``compress_kv_factor`` > 1, :1190-1208), joint image training (``use_image_num``), non-trivial latent
+State-dict compatible with the reference / HF ``LanguageBind/Open-Sora-Plan-v1.1.0`` transformer.  Not built: joint image
+training (``use_image_num``), non-trivial latent
 attention masks (the pipeline passes all-ones, pipeline_open_sora_plan.py:1119).  The diffusers leaf classes the
 reference file imports (GELU, Timesteps, TimestepEmbedding) are restated from their published semantics.
 """
@@ -66,8 +72,10 @@ class LatteT2V(nn.Module):
         super().__init__()
         if norm_type != "ada_norm_single" or activation_fn != "gelu-approximate" or norm_elementwise_affine:
             raise NotImplementedError("vsb200 Open-Sora-Plan v1.1.0 implements the released configuration (ada_norm_single, tanh-GELU)")
-        if compress_kv_factor != 1:
-            raise NotImplementedError("KV compression (compress_kv_factor > 1) is not built")
+        if int(compress_kv_factor) != compress_kv_factor or compress_kv_factor < 1:
+            raise ValueError(f"compress_kv_factor must be a positive integer, got {compress_kv_factor}")
+        if compress_kv_factor != 1 and use_rope:  # reference :2200
+            raise ValueError("KV compression (compress_kv_factor > 1) and RoPE cannot both be enabled")
         if rope_scaling_type != "linear":
             raise ValueError(f"Unknown RoPE scaling type {rope_scaling_type}")  # reference :1150
         if isinstance(sample_size, int):
@@ -94,6 +102,15 @@ class LatteT2V(nn.Module):
         stack = LatteBlockStack(dim, num_attention_heads, num_layers)
         self.transformer_blocks = stack.transformer_blocks
         self.temporal_transformer_blocks = stack.temporal_transformer_blocks
+        self.compress_kv_factor = k = int(compress_kv_factor)
+        if k != 1:  # second-half blocks, spatial and temporal (:2283-2320); layers and init as _init_compress (:1101-1122)
+            for d in range(num_layers // 2, num_layers):
+                for blk, sr in ((self.transformer_blocks[d], nn.Conv2d(dim, dim, k, stride=k, groups=dim)),
+                                (self.temporal_transformer_blocks[d], nn.Conv1d(dim, dim, k, stride=k, groups=dim))):
+                    sr.weight.data.fill_(1 / k ** (sr.weight.ndim - 2))
+                    sr.bias.data.zero_()
+                    blk.attn1.sr = sr
+                    blk.attn1.norm = nn.LayerNorm(dim)
         self._stack = [stack]
         self.scale_shift_table = nn.Parameter(torch.randn(2, dim) / dim**0.5)
         self.proj_out = nn.Linear(dim, patch_size * patch_size * out_channels)
@@ -160,6 +177,11 @@ class LatteT2V(nn.Module):
         h, w = H // p, W // p
         S = h * w
         L = encoder_hidden_states.shape[1]
+        k = self.compress_kv_factor
+        pad_t = k - 1 if Fr % 2 == 1 else 0  # the temporal compression prepends frame 0 for an odd frame count (:1190-1192)
+        if k != 1 and (h < k or w < k or (Fr + pad_t) < k):
+            raise ValueError(f"KV compression by {k} needs at least {k} patches per axis and {k} frames, got {h}x{w} patches and "
+                             f"{Fr} frames (+{pad_t} padding)")
         lens = text_lens(encoder_attention_mask, B, L)
         if (h, w) == self._grid and S == self.pos_table.shape[1]:
             pos = self.pos_table
@@ -181,7 +203,7 @@ class LatteT2V(nn.Module):
             tpe = comm.split_sequence(tpe, pm.sp_group, dim=1, pad=comm.get_pad("temporal"))
             Fr = x.shape[1]
         x = self._stack[0](x, enc, t6, tpe, ts_int=ts_int, all_timesteps=all_timesteps, sp_group=pm.sp_group if sp else None,
-                           rope=rope, enc_lens=lens)
+                           rope=rope, enc_lens=lens, kv_grid=(h, w), kv_pad_t=pad_t)
         y = ada_norm_single_out(self.scale_shift_table, embedded, x.view(B, Fr * S, C), B, Fr, S, self.eps)
         y = K.gemm_bias_act(y, self.proj_out.weight, self.proj_out.bias)  # [B, F*S, p*p*Cout]
         if sp:
