@@ -252,6 +252,35 @@ int vsb_ipc_get_handle(void* devptr, void* out_handle64);
 int vsb_ipc_open_handle(const void* handle64, void** out_devptr);
 int vsb_ipc_close_handle(void* devptr);
 
+/* ---- CogVideoX VAE decoder (models/autoencoders/autoencoder_kl_cogvideox.py) -------------------------------------
+ * Activations are channels-last [B, T, H, W, C] 16-bit tensors.
+ *
+ * vsb_vae_conv3d: CogVideoXCausalConv3d (:59-135, kernel (kt, 3, 3), kt = 3) and the up-sampler's Conv2d (kt = 1,
+ *   modules/upsampling.py:36,62-65) as an implicit GEMM on wgmma.  x [B, kt-1+T, H, W, Cin] holds the kt-1 causal context
+ *   frames first (copies of frame 0 or the carried conv_cache, :112-117); out [B, T, H, W, Cout].  The spatial zero
+ *   padding (:131-132) is not materialised.  w_packed [Cout_pad, kt*9, Cin_pad] is the weight packed tap-major (tap =
+ *   (dt*3 + dy)*3 + dx), Cin_pad / Cout_pad = Cin / Cout rounded up to a multiple of 64,
+ *   zero padded.  out = bf16(conv + bias) [+ resid, rounded again: the ResNet sum of :298]; round_conv = 1 rounds the
+ *   convolution to 16 bits before the bias is added.  Cin = 16 or a multiple of 64; Cout = 3 or a multiple of 64.
+ * vsb_vae_groupnorm_stats: mean and rstd = rsqrt(var + eps) (fp32, stats [B, G, 2]) of nn.GroupNorm over x [B, P, C]
+ *   (P = T*H*W pixels).  workspace: B * VSB_GN_CHUNKS * C * 2 floats.  Fixed-order reduction, no atomics: repeated
+ *   launches are bit-identical.  C in {64, 128, 256, 512}, G | C.
+ * vsb_vae_spatial_norm_silu: silu(GroupNorm(f) * conv_y(zq) + conv_b(zq)) (CogVideoXSpatialNorm3D :165-178, then the
+ *   ResNet's nonlinearity :280,:291 or conv_act :867), each eager op rounded.  zyb [B, Tz, h, w, 2C] holds conv_y | conv_b
+ *   at latent resolution, gathered with F.interpolate's nearest rule (the odd frame count split of :166-174).  The result
+ *   goes to frames t_off .. t_off+T-1 of out [B, T_out, H, W, C] (the next convolution's input after its context).
+ * vsb_vae_upsample2x: nearest 2x in H and W, and in T when compress_time (with the odd-frame rule of upsampling.py:40-60):
+ *   x [B, T, H, W, C] -> out [B, T2, 2H, 2W, C], T2 = T, 2T (even T > 1) or 2T - 1 (odd T > 1). */
+#define VSB_GN_CHUNKS 256
+int vsb_vae_conv3d(const vsb_bf16* x, const vsb_bf16* w_packed, const vsb_bf16* bias, const vsb_bf16* resid, vsb_bf16* out,
+                   int B, int T, int H, int W, int Cin, int Cout, int kt, int round_conv, void* stream);
+int vsb_vae_groupnorm_stats(const vsb_bf16* x, float* stats, float* workspace, int B, long long P, int C, int G, float eps,
+                            void* stream);
+int vsb_vae_spatial_norm_silu(const vsb_bf16* f, const float* stats, const vsb_bf16* gamma, const vsb_bf16* beta,
+                              const vsb_bf16* zyb, vsb_bf16* out, int B, int T, int H, int W, int C, int G, int Tz, int h,
+                              int w, int t_off, int T_out, void* stream);
+int vsb_vae_upsample2x(const vsb_bf16* x, vsb_bf16* out, int B, int T, int H, int W, int C, int compress_time, void* stream);
+
 /* ---- IEEE fp16 twins ----------------------------------------------------------------------------------------------
  * The reference runs CogVideoX-2b and Latte in torch.float16 (pipelines/cogvideox/pipeline_cogvideox.py:138-139,
  * pipelines/latte/pipeline_latte.py:201).  Every kernel entry above that touches activations exists a second time with
@@ -304,6 +333,15 @@ int vsb_dwconv_ffn_f16(const vsb_f16* h, const vsb_f16* w_taps, const vsb_f16* b
 int vsb_kv_compress_f16(const vsb_f16* x, const vsb_f16* w_taps, const vsb_f16* bias, const vsb_f16* ln_w, const vsb_f16* ln_b,
                         vsb_f16* out, int B, int T, int H, int W, int C, int kt, int kh, int kw, int pad_t, float eps,
                         int round_conv, void* stream);
+int vsb_vae_conv3d_f16(const vsb_f16* x, const vsb_f16* w_packed, const vsb_f16* bias, const vsb_f16* resid, vsb_f16* out,
+                       int B, int T, int H, int W, int Cin, int Cout, int kt, int round_conv, void* stream);
+int vsb_vae_groupnorm_stats_f16(const vsb_f16* x, float* stats, float* workspace, int B, long long P, int C, int G,
+                                float eps, void* stream);
+int vsb_vae_spatial_norm_silu_f16(const vsb_f16* f, const float* stats, const vsb_f16* gamma, const vsb_f16* beta,
+                                  const vsb_f16* zyb, vsb_f16* out, int B, int T, int H, int W, int C, int G, int Tz, int h,
+                                  int w, int t_off, int T_out, void* stream);
+int vsb_vae_upsample2x_f16(const vsb_f16* x, vsb_f16* out, int B, int T, int H, int W, int C, int compress_time,
+                           void* stream);
 
 #ifdef __cplusplus
 }

@@ -257,6 +257,79 @@ def kv_compress(x, w_taps, bias, ln_w, ln_b, B, T, H, W, window, pad_t=0, eps=1e
     return out
 
 
+VAE_GN_CHUNKS = 256  # VSB_GN_CHUNKS of include/vsb200.h
+
+
+def vae_conv3d(x, w_packed, bias, cout, kt, resid=None, round_conv=True):
+    """Causal (kt, 3, 3) convolution of x [B, kt-1+T, H, W, Cin] (causal context first, channels-last) with zero spatial
+    padding; w_packed [Cout_pad, kt*9, Cin_pad] tap-major (pack_conv_weight); returns [B, T, H, W, cout] = conv + bias
+    [+ resid].  round_conv: round the convolution before the bias is added (torch's cuDNN path)."""
+    lib, st = _prep(x, w_packed, bias, resid)
+    _bf16(x, "x")
+    _same_dtype(x, w_packed, bias, resid)
+    B, Tin, H, W, Cin = x.shape
+    T = Tin - (kt - 1)
+    out = torch.empty(B, T, H, W, cout, dtype=x.dtype, device=x.device)
+    with _Timed("vae_conv3d", 2 * B * T * H * W * cout * Cin * kt * 9):
+        _lib.check(_fn(lib, "vsb_vae_conv3d", x)(_p(x), _p(w_packed), _p(bias), _p(resid), _p(out), B, T, H, W, Cin, cout, kt,
+                                                 int(bool(round_conv)), st), "vae_conv3d")
+    return out
+
+
+def pack_conv_weight(w):
+    """[Cout, Cin, (kt,) 3, 3] conv weight -> [Cout_pad, kt*9, Cin_pad] tap-major, Cout and Cin zero padded to multiples
+    of 64 (include/vsb200.h)."""
+    if w.dim() == 4:
+        w = w[:, :, None]
+    cout, cin, kt = w.shape[0], w.shape[1], w.shape[2]
+    cout_pad, cin_pad = -(-cout // 64) * 64, -(-cin // 64) * 64
+    p = torch.zeros(cout_pad, kt * 9, cin_pad, dtype=w.dtype, device=w.device)
+    p[:cout, :, :cin] = w.permute(0, 2, 3, 4, 1).reshape(cout, kt * 9, cin)
+    return p
+
+
+def vae_groupnorm_stats(x, groups, eps):
+    """fp32 [B, groups, 2] (mean, rstd) of nn.GroupNorm over x [B, T, H, W, C] (channels-last)."""
+    lib, st = _prep(x)
+    _bf16(x, "x")
+    B, C = x.shape[0], x.shape[-1]
+    P = x.numel() // (B * C)
+    stats = torch.empty(B, groups, 2, dtype=torch.float32, device=x.device)
+    ws = torch.empty(B * VAE_GN_CHUNKS * C * 2, dtype=torch.float32, device=x.device)
+    with _Timed("vae_groupnorm_stats", x.numel() * 2):
+        _lib.check(_fn(lib, "vsb_vae_groupnorm_stats", x)(_p(x), _p(stats), _p(ws), B, P, C, groups, float(eps), st),
+                   "vae_groupnorm_stats")
+    return stats
+
+
+def vae_spatial_norm_silu(f, stats, gamma, beta, zyb, out, t_off=0):
+    """silu(GroupNorm(f) * zy + zb) of f [B, T, H, W, C] into frames t_off .. t_off+T-1 of out [B, T_out, H, W, C]; zyb
+    [B, Tz, h, w, 2C] = conv_y | conv_b of the latent, gathered with F.interpolate's nearest rule; stats from
+    vae_groupnorm_stats."""
+    lib, st = _prep(f, stats, gamma, beta, zyb, out)
+    _bf16(f, "f")
+    _same_dtype(f, gamma, beta, zyb, out)
+    B, T, H, W, C = f.shape
+    _, Tz, h, w, _ = zyb.shape
+    G = stats.shape[1]
+    with _Timed("vae_spatial_norm_silu", (2 * f.numel() + zyb.numel()) * 2):
+        _lib.check(_fn(lib, "vsb_vae_spatial_norm_silu", f)(_p(f), _p(stats), _p(gamma), _p(beta), _p(zyb), _p(out), B, T, H, W, C,
+                                                            G, Tz, h, w, t_off, out.shape[1], st), "vae_spatial_norm_silu")
+    return out
+
+
+def vae_upsample2x(x, compress_time):
+    """Nearest 2x of x [B, T, H, W, C] in H and W, and in T when compress_time (first frame kept single for odd T)."""
+    lib, st = _prep(x)
+    _bf16(x, "x")
+    B, T, H, W, C = x.shape
+    T2 = (2 * T - (T % 2)) if (compress_time and T > 1) else T
+    out = torch.empty(B, T2, 2 * H, 2 * W, C, dtype=x.dtype, device=x.device)
+    with _Timed("vae_upsample2x", (x.numel() + out.numel()) * 2):
+        _lib.check(_fn(lib, "vsb_vae_upsample2x", x)(_p(x), _p(out), B, T, H, W, C, int(bool(compress_time)), st), "vae_upsample2x")
+    return out
+
+
 def qk_rmsnorm_(qkv, wq, wk, H, D, eps=1e-6, rope_cos=None, rope_sin=None, pos_div=1, pos_mod=1):
     """In-place per-head RMSNorm of q and k; with rope tables also RoPE at position (row // pos_div) % pos_mod."""
     lib, st = _prep(qkv, wq, wk, rope_cos, rope_sin)

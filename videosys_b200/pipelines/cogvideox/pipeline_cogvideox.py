@@ -1,10 +1,15 @@
 """CogVideoX pipeline surface (mirror of videosys/pipelines/cogvideox/pipeline_cogvideox.py: CogVideoXPABConfig :33-44,
 CogVideoXConfig :47-112, CogVideoXPipeline.generate :489-737) around the native CogVideoXTransformer3DModel.
 
-In scope: the config classes, ``generate()``'s signature and shape rules, the CFG + DDIM denoising loop (:692-733) and
-the denoiser.  Out of scope as for OpenSora (SURVEY.md 2.1): T5 encoder, VAE decode (once per video) -- pass
-``prompt_embeds`` / ``negative_prompt_embeds`` or a ``text_encoder_fn``; without a ``vae_decode_fn`` the LATENTS are
-returned (``output_type="latent"`` semantics).  dtype follows the reference: fp16 for "THUDM/CogVideoX-2b", else bf16.
+In scope: the config classes, ``generate()``'s signature and shape rules, the CFG + DDIM denoising loop (:692-733),
+the denoiser, and -- opt-in through ``CogVideoXConfig(vae=...)`` -- the VAE decode tail (:359-364, :739-741) on the native
+decoder (models/autoencoders/autoencoder_kl_cogvideox.py).  Out of scope as for OpenSora (SURVEY.md 2.1): the T5 encoder
+-- pass ``prompt_embeds`` / ``negative_prompt_embeds`` or a ``text_encoder_fn``.  Without a ``vae`` or a ``vae_decode_fn``
+the LATENTS are returned (``output_type="latent"`` semantics).  dtype follows the reference: fp16 for
+"THUDM/CogVideoX-2b", else bf16.
+
+The video post-processing restates diffusers' ``VideoProcessor.postprocess_video`` (diffusers is not a dependency):
+``(x / 2 + 0.5).clamp(0, 1)`` per frame, then "pt" -> [B, F, 3, H, W], "np" -> [B, F, H, W, 3], "pil" -> lists of PIL images.
 """
 import zlib
 from typing import Callable, Optional
@@ -27,7 +32,7 @@ class CogVideoXConfig:
     def __init__(self, model_path: str = "THUDM/CogVideoX-2b", num_gpus: int = 1, cpu_offload: bool = False,
                  vae_tiling: bool = True, enable_pab: bool = False, pab_config=None,
                  transformer_config: Optional[dict] = None, state_dict=None, text_encoder_fn: Optional[Callable] = None,
-                 vae_decode_fn: Optional[Callable] = None):
+                 vae_decode_fn: Optional[Callable] = None, vae=None):
         self.model_path = model_path
         self.pipeline_cls = CogVideoXPipeline
         self.num_gpus = num_gpus
@@ -40,6 +45,8 @@ class CogVideoXConfig:
         self.state_dict = state_dict
         self.text_encoder_fn = text_encoder_fn
         self.vae_decode_fn = vae_decode_fn
+        # native VAE decoder: a local snapshot directory (its root or its vae/ folder) or an AutoencoderKLCogVideoX
+        self.vae = vae
 
 
 class CogVideoXPipeline(ParallelPipelineMixin):
@@ -67,9 +74,44 @@ class CogVideoXPipeline(ParallelPipelineMixin):
             self.transformer.load_state_dict(config.state_dict)
         self.transformer = self.transformer.to(self._device).eval()
         self.scheduler = CogVideoXDDIMScheduler()
+        self.vae = self._load_vae()
         if config.enable_pab:
             set_pab_manager(config.pab_config)
         self._set_parallel()
+
+    def _load_vae(self):
+        """The native decoder of ``config.vae`` in the pipeline dtype, with tiling as the reference sets it (:170-172)."""
+        import os
+
+        from ...models.autoencoders.autoencoder_kl_cogvideox import AutoencoderKLCogVideoX
+
+        v = self._config.vae
+        if v is None:
+            return None
+        if not isinstance(v, AutoencoderKLCogVideoX):
+            v = str(v)
+            v = AutoencoderKLCogVideoX.from_pretrained(v, subfolder="vae" if os.path.isdir(os.path.join(v, "vae")) else "")
+        v = v.to(self._dtype).to(self._device).eval()
+        if self._config.vae_tiling:
+            v.enable_tiling()
+        return v
+
+    def decode_latents_to_video(self, latents, output_type: str = "pil"):
+        """Reference decode_latents (:359-364) and VideoProcessor.postprocess_video: latents [B, F, C, h, w]."""
+        z = latents.permute(0, 2, 1, 3, 4)
+        z = 1 / self.vae.config.scaling_factor * z
+        frames = self.vae.decode(z).sample  # [B, 3, F, H, W]
+        video = (frames / 2 + 0.5).clamp(0, 1).permute(0, 2, 1, 3, 4)  # [B, F, 3, H, W]
+        if output_type == "pt":
+            return video
+        arr = video.permute(0, 1, 3, 4, 2).float().cpu().numpy()  # [B, F, H, W, 3]
+        if output_type == "np":
+            return arr
+        if output_type == "pil":
+            from PIL import Image
+
+            return [[Image.fromarray((f * 255).round().astype("uint8")) for f in clip] for clip in arr]
+        raise ValueError(f"output_type={output_type!r}: expected 'pil', 'np', 'pt' or 'latent'")
 
     def _embeds(self, prompt, negative_prompt, max_sequence_length):
         cfg = self.transformer.config
@@ -160,6 +202,8 @@ class CogVideoXPipeline(ParallelPipelineMixin):
             lat = self.scheduler.step(noise, t, lat, eta=eta)[0].to(dt)
         if self._config.vae_decode_fn is not None and output_type != "latent":
             video = self._config.vae_decode_fn(lat)
+        elif self.vae is not None and output_type != "latent":
+            video = self.decode_latents_to_video(lat, output_type)
         else:
             video = lat.float().cpu()  # latents: the VAE is out of scope
         return VideoSysPipelineOutput(video=video) if return_dict else (video,)
