@@ -281,6 +281,38 @@ int vsb_vae_spatial_norm_silu(const vsb_bf16* f, const float* stats, const vsb_b
                               int w, int t_off, int T_out, void* stream);
 int vsb_vae_upsample2x(const vsb_bf16* x, vsb_bf16* out, int B, int T, int H, int W, int C, int compress_time, void* stream);
 
+/* ---- Open-Sora-Plan causal-VAE decoder (models/autoencoders/autoencoder_kl_open_sora_plan.py) ---------------------
+ * Channels-last [B, T, H, W, C] 16-bit activations; the causal convolutions run on vsb_vae_conv3d, the 1x1x1 ones and
+ * the attention's S = Q K^T and O = P V on vsb_gemm_bias_act / vsb_gemm_bias_residual.
+ *
+ * vsb_vae_groupnorm_act: Normalize = nn.GroupNorm(G, C, eps=1e-6) of x (stats from vsb_vae_groupnorm_stats, kept in the
+ *   16-bit dtype as torch does), then with act = 1 the nonlinearity x * torch.sigmoid(x) (v1.2.0 :100-101, v1.1.0
+ *   :1255-1256), each eager op rounded.  Writes frames t_off .. t_off+T-1 of out [B, T_out, H, W, C].  C % 8 == 0, G | C.
+ * vsb_vae_upsample_linear2x: F.interpolate(mode="trilinear", align_corners=False) of x [B, T, H, W, C] by 2 in H and W
+ *   (spatial) and by 2 in T over frames 1.. with frame 0 kept (temporal; Spatial2xTime2x3DUpsample v1.2.0 :349-357,
+ *   TimeUpsample2x / TimeUpsampleRes2x v1.1.0 :1549-1596), fp32, rounded once.  To = 1 + 2 (T - 1) frames when temporal
+ *   and T > 1, else T, written to frames t_off .. t_off+To-1 of out [B, T_out, Ho, Wo, C].  C % 8 == 0.
+ * vsb_vae_mix: out = alpha * x + one_minus_alpha * y with each product and the sum rounded (TimeUpsampleRes2x :1596);
+ *   x = frames t_off .. t_off+T-1 of xbuf [B, T_x, n], y and out [B, T, n], n = H*W*C, n % 8 == 0.
+ * vsb_vae_attn_split: the attention block's fused q | k | v (qkv [B, T, P, 3C], P = H*W) to per-frame GEMM operands
+ *   q [B*T, P, C], k [B*T, Pp, C] and vt [B*T, C, Pp] (V transposed), zero past P (Pp = P rounded up to 8).  mixed = 0:
+ *   AttnBlock3DFix (frames as they are); mixed = 1: AttnBlock3D's reshape(b*t, c, h*w) of a b c t h w tensor
+ *   (v1.1.0 :921-929): pseudo-frame j, channel ch reads channel (j*C + ch) / T of frame (j*C + ch) % T.  C % 32 == 0.
+ * vsb_vae_attn_softmax: in place on S [rows, Pp]: softmax over the first P columns of bf16(S * scale) in fp32, rounded
+ *   once (torch.nn.functional.softmax of w_ * c ** -0.5); columns P .. Pp-1 become zero.
+ * vsb_vae_attn_merge: AttnBlock3D's output h_.reshape(b, c, t, h, w) (:932): out [B, T, P, C] channel c, frame t =
+ *   o [B*T, P, C] pseudo-frame (c*T + t) / C, channel (c*T + t) % C. */
+int vsb_vae_groupnorm_act(const vsb_bf16* x, const float* stats, const vsb_bf16* gamma, const vsb_bf16* beta, vsb_bf16* out,
+                          int B, int T, int H, int W, int C, int G, int t_off, int T_out, int act, void* stream);
+int vsb_vae_upsample_linear2x(const vsb_bf16* x, vsb_bf16* out, int B, int T, int H, int W, int C, int spatial, int temporal,
+                              int t_off, int T_out, void* stream);
+int vsb_vae_mix(const vsb_bf16* xbuf, const vsb_bf16* y, vsb_bf16* out, int B, int T, long long n, int t_off, int T_x,
+                float alpha, float one_minus_alpha, void* stream);
+int vsb_vae_attn_split(const vsb_bf16* qkv, vsb_bf16* q, vsb_bf16* k, vsb_bf16* vt, int B, int T, int P, int Pp, int C,
+                       int mixed, void* stream);
+int vsb_vae_attn_softmax(vsb_bf16* S, int rows, int P, int Pp, float scale, void* stream);
+int vsb_vae_attn_merge(const vsb_bf16* o, vsb_bf16* out, int B, int T, int P, int C, void* stream);
+
 /* ---- IEEE fp16 twins ----------------------------------------------------------------------------------------------
  * The reference runs CogVideoX-2b and Latte in torch.float16 (pipelines/cogvideox/pipeline_cogvideox.py:138-139,
  * pipelines/latte/pipeline_latte.py:201).  Every kernel entry above that touches activations exists a second time with
@@ -342,6 +374,16 @@ int vsb_vae_spatial_norm_silu_f16(const vsb_f16* f, const float* stats, const vs
                                   int w, int t_off, int T_out, void* stream);
 int vsb_vae_upsample2x_f16(const vsb_f16* x, vsb_f16* out, int B, int T, int H, int W, int C, int compress_time,
                            void* stream);
+int vsb_vae_groupnorm_act_f16(const vsb_f16* x, const float* stats, const vsb_f16* gamma, const vsb_f16* beta, vsb_f16* out,
+                              int B, int T, int H, int W, int C, int G, int t_off, int T_out, int act, void* stream);
+int vsb_vae_upsample_linear2x_f16(const vsb_f16* x, vsb_f16* out, int B, int T, int H, int W, int C, int spatial,
+                                  int temporal, int t_off, int T_out, void* stream);
+int vsb_vae_mix_f16(const vsb_f16* xbuf, const vsb_f16* y, vsb_f16* out, int B, int T, long long n, int t_off, int T_x,
+                    float alpha, float one_minus_alpha, void* stream);
+int vsb_vae_attn_split_f16(const vsb_f16* qkv, vsb_f16* q, vsb_f16* k, vsb_f16* vt, int B, int T, int P, int Pp, int C,
+                           int mixed, void* stream);
+int vsb_vae_attn_softmax_f16(vsb_f16* S, int rows, int P, int Pp, float scale, void* stream);
+int vsb_vae_attn_merge_f16(const vsb_f16* o, vsb_f16* out, int B, int T, int P, int C, void* stream);
 
 #ifdef __cplusplus
 }

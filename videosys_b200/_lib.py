@@ -48,6 +48,12 @@ SIGNATURES = {
     "vsb_vae_groupnorm_stats": (_i, [_vp, _vp, _vp, _i, _ll, _i, _i, _f, _vp]),
     "vsb_vae_spatial_norm_silu": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "vsb_vae_upsample2x": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
+    "vsb_vae_groupnorm_act": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "vsb_vae_upsample_linear2x": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "vsb_vae_mix": (_i, [_vp, _vp, _vp, _i, _i, _ll, _i, _i, _f, _f, _vp]),
+    "vsb_vae_attn_split": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
+    "vsb_vae_attn_softmax": (_i, [_vp, _i, _i, _i, _f, _vp]),
+    "vsb_vae_attn_merge": (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),
     "vsb_tmap_cache_stats": (C.c_ulonglong, [_i]),
     "vsb_dsp_alloc": (_i, [C.POINTER(_vp), _sz]),
     "vsb_dsp_free": (_i, [_vp]),
@@ -61,7 +67,9 @@ F16_TWINS = ("vsb_ln_modulate", "vsb_ln_modulate_affine", "vsb_modulation_table"
              "vsb_qk_rmsnorm", "vsb_qk_rmsnorm_rope", "vsb_qk_rope_halves", "vsb_qk_layernorm", "vsb_attn_short", "vsb_gemm_bias_act",
              "vsb_gemm_bias_residual", "vsb_attn_flash", "vsb_attn_flash_strided", "vsb_patch_embed",
              "vsb_dwconv_shuffle", "vsb_gate_residual_unshuffle", "vsb_dwconv_ffn", "vsb_kv_compress",
-             "vsb_vae_conv3d", "vsb_vae_groupnorm_stats", "vsb_vae_spatial_norm_silu", "vsb_vae_upsample2x")
+             "vsb_vae_conv3d", "vsb_vae_groupnorm_stats", "vsb_vae_spatial_norm_silu", "vsb_vae_upsample2x",
+             "vsb_vae_groupnorm_act", "vsb_vae_upsample_linear2x", "vsb_vae_mix", "vsb_vae_attn_split", "vsb_vae_attn_softmax",
+             "vsb_vae_attn_merge")
 for _n in F16_TWINS:
     SIGNATURES[_n + "_f16"] = SIGNATURES[_n]
 

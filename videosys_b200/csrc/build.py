@@ -7,9 +7,9 @@ import subprocess
 import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-SOURCES = ["api.cu", "elementwise.cu", "attn_short.cu", "gemm_wgmma.cu", "attn_wgmma.cu", "attn_mma.cu", "dsp_p2p.cu", "patch_embed.cu", "dwconv.cu", "vae_conv.cu"]
+SOURCES = ["api.cu", "elementwise.cu", "attn_short.cu", "gemm_wgmma.cu", "attn_wgmma.cu", "attn_mma.cu", "dsp_p2p.cu", "patch_embed.cu", "dwconv.cu", "vae_conv.cu", "vae_osp.cu"]
 # every kernel file below is compiled twice: bf16 (as is) and IEEE fp16 (-DVSB_HALF -> *.f16.o, entries suffixed _f16)
-TWINNED = ["elementwise.cu", "attn_short.cu", "gemm_wgmma.cu", "attn_wgmma.cu", "attn_mma.cu", "patch_embed.cu", "dwconv.cu", "vae_conv.cu"]
+TWINNED = ["elementwise.cu", "attn_short.cu", "gemm_wgmma.cu", "attn_wgmma.cu", "attn_mma.cu", "patch_embed.cu", "dwconv.cu", "vae_conv.cu", "vae_osp.cu"]
 HEADERS = ["vsb_common.cuh", "vsb_host.h", "wgmma.cuh", "attn_params.cuh", "dsp_common.cuh", os.path.join("..", "..", "include", "vsb200.h")]
 LIB = os.path.join(HERE, "libvsb200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")

@@ -330,6 +330,86 @@ def vae_upsample2x(x, compress_time):
     return out
 
 
+def vae_groupnorm_act(x, stats, gamma, beta, out=None, t_off=0, act=True):
+    """GroupNorm of x [B, T, H, W, C] with stats from vae_groupnorm_stats, then x * sigmoid(x) when act, into frames
+    t_off .. t_off+T-1 of out [B, T_out, H, W, C] (default: a new [B, T, H, W, C])."""
+    lib, st = _prep(x, stats, gamma, beta, out)
+    _bf16(x, "x")
+    _same_dtype(x, gamma, beta, out)
+    B, T, H, W, C = x.shape
+    out = torch.empty_like(x) if out is None else out
+    with _Timed("vae_groupnorm_act", 2 * x.numel() * 2):
+        _lib.check(_fn(lib, "vsb_vae_groupnorm_act", x)(_p(x), _p(stats), _p(gamma), _p(beta), _p(out), B, T, H, W, C, stats.shape[1],
+                                                        t_off, out.shape[1], int(bool(act)), st), "vae_groupnorm_act")
+    return out
+
+
+def vae_upsample_linear2x(x, spatial, temporal, out=None, t_off=0):
+    """Trilinear (align_corners=False) 2x of x [B, T, H, W, C] in H and W (spatial) and in T over frames 1.. (temporal),
+    into frames t_off.. of out [B, T_out, Ho, Wo, C] (default: a new tensor of exactly the output frames)."""
+    lib, st = _prep(x, out)
+    _bf16(x, "x")
+    _same_dtype(x, out)
+    B, T, H, W, C = x.shape
+    To = 2 * T - 1 if (temporal and T > 1) else T
+    if out is None:
+        out = torch.empty(B, To, H * (2 if spatial else 1), W * (2 if spatial else 1), C, dtype=x.dtype, device=x.device)
+    with _Timed("vae_upsample_linear2x", (x.numel() + out.numel()) * 2):
+        _lib.check(_fn(lib, "vsb_vae_upsample_linear2x", x)(_p(x), _p(out), B, T, H, W, C, int(bool(spatial)), int(bool(temporal)),
+                                                            t_off, out.shape[1], st), "vae_upsample_linear2x")
+    return out
+
+
+def vae_mix(xbuf, y, alpha, one_minus_alpha, t_off=0):
+    """alpha * x + one_minus_alpha * y, each op rounded, x = frames t_off.. of xbuf [B, T_x, H, W, C], y [B, T, H, W, C]."""
+    lib, st = _prep(xbuf, y)
+    _same_dtype(xbuf, y)
+    B, T = y.shape[0], y.shape[1]
+    out = torch.empty_like(y)
+    with _Timed("vae_mix", 3 * y.numel() * 2):
+        _lib.check(_fn(lib, "vsb_vae_mix", y)(_p(xbuf), _p(y), _p(out), B, T, y[0, 0].numel(), t_off, xbuf.shape[1], float(alpha),
+                                              float(one_minus_alpha), st), "vae_mix")
+    return out
+
+
+def vae_attn_split(qkv, C, mixed):
+    """qkv [B, T, H, W, 3C] -> per-frame q [B*T, P, C], k [B*T, Pp, C], vt [B*T, C, Pp] (P = H*W, Pp = P rounded up to 8,
+    zero past P); mixed: AttnBlock3D's frame / channel mixing."""
+    lib, st = _prep(qkv)
+    _bf16(qkv, "qkv")
+    B, T = qkv.shape[0], qkv.shape[1]
+    P = qkv[0, 0].numel() // (3 * C)
+    Pp = -(-P // 8) * 8
+    q = torch.empty(B * T, P, C, dtype=qkv.dtype, device=qkv.device)
+    k = torch.empty(B * T, Pp, C, dtype=qkv.dtype, device=qkv.device)
+    vt = torch.empty(B * T, C, Pp, dtype=qkv.dtype, device=qkv.device)
+    with _Timed("vae_attn_split", 2 * qkv.numel() * 2):
+        _lib.check(_fn(lib, "vsb_vae_attn_split", qkv)(_p(qkv), _p(q), _p(k), _p(vt), B, T, P, Pp, C, int(bool(mixed)), st),
+                   "vae_attn_split")
+    return q, k, vt
+
+
+def vae_attn_softmax_(S, P, scale):
+    """In place: softmax over the first P columns of bf16(S * scale), S [rows, Pp]; columns P.. become zero."""
+    lib, st = _prep(S)
+    _bf16(S, "S")
+    rows, Pp = S.numel() // S.shape[-1], S.shape[-1]
+    with _Timed("vae_attn_softmax", 2 * S.numel() * 2):
+        _lib.check(_fn(lib, "vsb_vae_attn_softmax", S)(_p(S), rows, P, Pp, float(scale), st), "vae_attn_softmax")
+    return S
+
+
+def vae_attn_merge(o, B, T, H, W):
+    """AttnBlock3D's output scatter: o [B*T, P, C] (pseudo-frames) -> [B, T, H, W, C]."""
+    lib, st = _prep(o)
+    _bf16(o, "o")
+    C = o.shape[-1]
+    out = torch.empty(B, T, H, W, C, dtype=o.dtype, device=o.device)
+    with _Timed("vae_attn_merge", 2 * o.numel() * 2):
+        _lib.check(_fn(lib, "vsb_vae_attn_merge", o)(_p(o), _p(out), B, T, H * W, C, st), "vae_attn_merge")
+    return out
+
+
 def qk_rmsnorm_(qkv, wq, wk, H, D, eps=1e-6, rope_cos=None, rope_sin=None, pos_div=1, pos_mod=1):
     """In-place per-head RMSNorm of q and k; with rope tables also RoPE at position (row // pos_div) % pos_mod."""
     lib, st = _prep(qkv, wq, wk, rope_cos, rope_sin)

@@ -1,2 +1,3 @@
-"""VAE decoders (videosys/models/autoencoders): the CogVideoX decoder on sm_90a kernels."""
+"""VAE decoders (videosys/models/autoencoders): the CogVideoX and Open-Sora-Plan decoders on sm_90a kernels."""
 from .autoencoder_kl_cogvideox import AutoencoderKLCogVideoX  # noqa: F401
+from .autoencoder_kl_open_sora_plan import CausalVAEModelV110, CausalVAEModelV120  # noqa: F401

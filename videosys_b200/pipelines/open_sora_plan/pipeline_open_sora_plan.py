@@ -6,9 +6,13 @@ Version v110 (``LatteT2V``, 65 or 221 frames at 512 x 512, head_dim 72): CFG bat
 warm-up: the transformer is evaluated at every entry of ``scheduler.timesteps``), learned-sigma split, PAB with the MLP skip.
 Version v120 (``OpenSoraT2V``, 29 or 93 frames at 480p / 720p, head_dim 96, 3-D RoPE): ancestral Euler steps (the latent is
 scaled by the scheduler before every forward, :1097), PAB with the spatial and the cross gate; its attention runs on the
-warp-level kernel of csrc/attn_mma.cu (head_dim 64 / 72 run on csrc/attn_wgmma.cu).  Out of scope as for the other pipelines (SURVEY.md 2.1): T5 encoder and the
-causal VAE -- pass ``prompt_embeds`` (+ masks) or a ``text_encoder_fn``; without a ``vae_decode_fn`` the LATENTS are returned.
-dtype fp16 as the reference (:262).
+warp-level kernel of csrc/attn_mma.cu (head_dim 64 / 72 run on csrc/attn_wgmma.cu).
+
+Opt-in through ``OpenSoraPlanConfig(vae=...)``: the causal-VAE decode tail (:1168-1191) on the native decoder of the
+version (models/autoencoders/autoencoder_kl_open_sora_plan.py), tiled with the reference's sizes when ``enable_tiling``
+(:309-315), then ``((v / 2 + 0.5).clamp(0, 1) * 255).to(uint8)`` as ``[B, T, H, W, 3]``, cut to the requested frames and
+size.  Out of scope as for the other pipelines (SURVEY.md 2.1): the T5 encoder -- pass ``prompt_embeds`` (+ masks) or a
+``text_encoder_fn``.  Without a ``vae`` or a ``vae_decode_fn`` the LATENTS are returned.  dtype fp16 as the reference (:262).
 """
 import math
 import zlib
@@ -52,7 +56,8 @@ class OpenSoraPlanConfig:
     def __init__(self, version: str = "v120", transformer_type: str = "29x480p", transformer: str = None, text_encoder: str = None,
                  num_gpus: int = 1, cpu_offload: bool = False, enable_tiling: bool = True, tile_overlap_factor: float = 0.25,
                  enable_pab: bool = False, pab_config: PABConfig = None, transformer_config: Optional[dict] = None,
-                 state_dict=None, text_encoder_fn: Optional[Callable] = None, vae_decode_fn: Optional[Callable] = None):
+                 state_dict=None, text_encoder_fn: Optional[Callable] = None, vae_decode_fn: Optional[Callable] = None,
+                 vae=None):
         self.pipeline_cls = OpenSoraPlanPipeline
         assert version in ["v110", "v120"], f"Unknown Open-Sora-Plan version: {version}"
         self.version, self.transformer_type = version, transformer_type
@@ -72,6 +77,8 @@ class OpenSoraPlanConfig:
         # native build extras: architecture / weights / out-of-scope stages supplied by the caller
         self.transformer_config, self.state_dict = transformer_config, state_dict
         self.text_encoder_fn, self.vae_decode_fn = text_encoder_fn, vae_decode_fn
+        # native VAE decoder: a local snapshot directory (its root or its vae/ folder) or a decoder instance of the version
+        self.vae = vae
 
 
 class OpenSoraPlanPipeline(ParallelPipelineMixin):
@@ -97,9 +104,39 @@ class OpenSoraPlanPipeline(ParallelPipelineMixin):
             self.transformer.load_state_dict(config.state_dict)
         self.transformer = self.transformer.to(self._device).eval()
         self.scheduler = PNDMScheduler() if config.version == "v110" else EulerAncestralDiscreteScheduler()
+        self.vae = self._load_vae()
         if config.enable_pab:
             set_pab_manager(config.pab_config)
         self._set_parallel()
+
+    def _load_vae(self):
+        """The native decoder of ``config.vae`` in the pipeline dtype, with the reference's tiling settings (:309-315)."""
+        import os
+
+        from ...models.autoencoders.autoencoder_kl_open_sora_plan import decoder_class
+
+        cls = decoder_class(self._config.version)
+        v = self._config.vae
+        if v is None:
+            return None
+        if not isinstance(v, cls):
+            v = str(v)
+            v = cls.from_pretrained(v, subfolder="vae" if os.path.isdir(os.path.join(v, "vae")) else None)
+        v = v.to(self._dtype).to(self._device).eval()
+        if self._config.enable_tiling:
+            v.enable_tiling()
+            v.tile_overlap_factor = self._config.tile_overlap_factor
+            v.tile_sample_min_size = 512
+            v.tile_latent_min_size = 64
+            v.tile_sample_min_size_t = 29
+            v.tile_latent_min_size_t = 8
+        return v
+
+    def decode_latents(self, latents):
+        """Reference decode_latents (:1184-1191) with CausalVAEModelWrapper.decode: latents [B, C, T, h, w] ->
+        uint8 [B, T', H, W, 3]."""
+        video = self.vae.decode(latents.to(self.vae.dtype) / 0.18215).permute(0, 2, 1, 3, 4)  # b t c h w
+        return ((video / 2.0 + 0.5).clamp(0, 1) * 255).to(dtype=torch.uint8).cpu().permute(0, 1, 3, 4, 2).contiguous()
 
     @classmethod
     def latent_frames(cls, num_frames: int) -> int:
@@ -176,6 +213,8 @@ class OpenSoraPlanPipeline(ParallelPipelineMixin):
             lat = self.scheduler.step(noise, t, lat)[0].to(dt)
         if self._config.vae_decode_fn is not None and output_type != "latents":
             video = self._config.vae_decode_fn(lat)
+        elif getattr(self, "vae", None) is not None and output_type != "latents":
+            video = self.decode_latents(lat)[:, :self._config.num_frames, :height, :width]
         else:
             video = lat.float().cpu()  # latents: the VAE is out of scope
         return VideoSysPipelineOutput(video=video) if return_dict else (video,)
