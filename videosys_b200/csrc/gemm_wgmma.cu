@@ -1,14 +1,24 @@
 // vsb200 -- 16-bit TN GEMM on the Hopper warpgroup tensor cores: out[M,N] = act(A[M,K] @ W[N,K]^T + bias), or with the
 // residual branch fused into the epilogue: out = resid + [gate *] (A @ W^T + bias).
 //
-// One CTA per 128 x BN output tile, three warpgroups:
-//   warpgroup 0     TMA producer (one thread): A tile 128x64 and W tile BNx64, SWIZZLE_128B, kStages-deep mbarrier ring
-//   warpgroups 1-2  consumers: rows 0..63 / 64..127 of the tile, wgmma.m64nBNk16 straight from the swizzled stages into
-//                   fp32 registers; each consumer releases a stage once the wgmma that read it has retired
-//   epilogue        the consumers: + bias -> [bf16 round -> tanh-GELU | gate + residual] -> 16-bit -> 128B-swizzled
-//                   staging tile -> TMA store (64-column chunks)
-// Tiles are walked N-fastest so that the 128-row A panel is reused from L2 across its N tiles.  TMA zero-fills K/M/N
-// tails on load and clips them on store, so any M, N % 8 == 0, K % 8 == 0 is legal.
+// Two kernels, chosen in gemm_dispatch from the epilogue and K.  The gate + residual epilogue, and a GELU epilogue at
+// K <= 1536, run the persistent ping-pong kernel, which hides the epilogue under the tensor cores.  A bias-only GEMM,
+// and a GELU GEMM at longer K, run gemm_tile_kernel (one CTA per 128 x 192 tile, below), whose K loop is faster.
+//
+// Persistent ping-pong kernel: min(tiles, SMs) CTAs, each walking the 128 x 128 output tiles blockIdx.x, + gridDim.x, ...
+// N-fastest (so the 128-row A panel is reused from L2 across its N tiles), two warpgroups and one warp:
+//   warp 8          TMA producer (one thread): A tile 128x64 and W tile 128x64 per k-block,
+//                   SWIZZLE_128B, through a kStages-deep mbarrier ring whose position carries over from tile to tile, so
+//                   the loads of the next tile are in flight while the current one is still on the tensor cores; for the
+//                   fused residual also the tile's resid block, straight into the staging buffer of the consumer that owns it
+//   warpgroups 0-1  consumers, taking alternate tiles of the CTA: wgmma.m64n128k16 x 2 (rows 0..63
+//                   and 64..127) from the swizzled stages into 128 fp32 registers per thread.  The two mainloops take turns
+//                   on the tensor cores (named barriers 1 / 2), so one consumer's epilogue -- + bias -> [bf16 round ->
+//                   tanh-GELU | gate + residual] -> 16-bit -> its own 128B-swizzled staging tile -> TMA store -- runs under
+//                   the other consumer's mainloop, and so does the refill of the ring between tiles
+// A consumer releases a stage once the wgmma that read it has retired, and its staging tile once the TMA store has read
+// it (cp.async.bulk.wait_group.read).  TMA zero-fills K/M/N tails on load and clips them on store, so any M,
+// N % 8 == 0, K % 8 == 0 is legal.
 #include "vsb_common.cuh"
 #include "vsb_host.h"
 #include "wgmma.cuh"
@@ -16,17 +26,19 @@
 namespace vsb {
 
 constexpr int kBM = 128;
+constexpr int kBN = 128;
 constexpr int kBK = 64;
-constexpr int kGemmThreads = 384;
+constexpr int kPersistentGeluMaxK = 1536;  // longest K at which a GELU epilogue runs on the persistent kernel
+// two consumer warpgroups + one producer warp; ptxas allots 168 registers per thread: 128 accumulators + the epilogue
+constexpr int kGemmThreads = 288;
 
-template <int BN>
 struct GemmCfg {
   static constexpr int kABytes = kBM * kBK * 2;
-  static constexpr int kStageBytes = (kBM + BN) * kBK * 2;
-  static constexpr int kCBytes = kBM * BN * 2;
-  static constexpr int kStages = 4;
-  // + 1024 for manual alignment, + 256 for barriers
-  static constexpr int kSmemBytes = kStages * kStageBytes + kCBytes + 1024 + 256;
+  static constexpr int kStageBytes = (kBM + kBN) * kBK * 2;
+  static constexpr int kCBytes = kBM * kBN * 2;  // one staging tile: [kBN/64][128 rows][128 B] swizzled
+  static constexpr int kStages = 5;
+  // 5 x 32 KB ring + 2 x 32 KB staging, + 1024 for manual alignment, + 256 for barriers: 230 656 B of the 227 KB
+  static constexpr int kSmemBytes = kStages * kStageBytes + 2 * kCBytes + 1024 + 256;
 };
 
 __device__ __forceinline__ float gelu_tanh_f(float x) {
@@ -48,11 +60,28 @@ __device__ __forceinline__ float gelu_erf_f(float x) { return x * 0.5f * (1.f + 
 // ACT == 2: out = resid + g, g = bf16(gate * y) (gate_row >= 0, per-frame t/t0 select) or g = y (plain residual add),
 // y = bf16(acc + bias): the eager chain of open_sora_transformer_3d.py (Linear, gate multiply, residual add) in the epilogue.
 struct EpiArgs {
-  const bf16* resid;      // [M, N], may alias the output
+  const bf16* resid;      // [M, N], may alias the output; read by TMA through its own tensor map
   const bf16* mod;        // [2, B, 6, N] or null
   const uint8_t* x_mask;  // [B, T] or null
   int gate_row, B, T, S;
 };
+
+// ---- one CTA per 128 x BN tile (BN = 192 where it divides N): bias only, or GELU at long K --------------------------
+// Without an epilogue to hide, the persistent kernel's 128 x 128 tile loses to this one: its mainloop moves 32 KB from L2
+// per 2.1 MFLOP against 40 KB per 3.1 MFLOP here, and at ~8.7 TB/s both are bound by the L2 -> SM bandwidth, so the wider
+// tile runs the K loop ~20 % faster (DESIGN.md section 9).  Warpgroup 0 is the TMA producer (one thread), warpgroups 1-2
+// own rows 0..63 / 64..127 of the tile; the epilogue adds the bias, [rounds and applies tanh- or erf-GELU,] and
+// TMA-stores the 16-bit tile.
+template <int BN>
+struct TileCfg {
+  static constexpr int kABytes = kBM * kBK * 2;
+  static constexpr int kStageBytes = (kBM + BN) * kBK * 2;
+  static constexpr int kCBytes = kBM * BN * 2;
+  static constexpr int kStages = 4;
+  // + 1024 for manual alignment, + 256 for barriers
+  static constexpr int kSmemBytes = kStages * kStageBytes + kCBytes + 1024 + 256;
+};
+constexpr int kTileThreads = 384;
 
 template <int BN>
 __device__ __forceinline__ void wgmma_tile(float (&d)[BN / 2], uint64_t da, uint64_t db, uint32_t scale_d) {
@@ -63,11 +92,10 @@ __device__ __forceinline__ void wgmma_tile(float (&d)[BN / 2], uint64_t da, uint
 }
 
 template <int BN, int ACT>
-__global__ void __launch_bounds__(kGemmThreads, 1)
-gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_w,
-                  const __grid_constant__ CUtensorMap tm_c, const bf16* __restrict__ bias, int M, int N, int K,
-                  const EpiArgs ep) {
-  using Cfg = GemmCfg<BN>;
+__global__ void __launch_bounds__(kTileThreads, 1)
+gemm_tile_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_w,
+                 const __grid_constant__ CUtensorMap tm_c, const bf16* __restrict__ bias, int M, int N, int K) {
+  using Cfg = TileCfg<BN>;
   constexpr int kStages = Cfg::kStages;
   extern __shared__ unsigned char smem_dyn[];
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~uintptr_t(1023));
@@ -94,7 +122,6 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
   __syncthreads();
 
   if (wg == 0) {
-    // ===================== TMA producer =====================
     if (threadIdx.x == 0) {
       for (int kb = 0; kb < num_kb; ++kb) {
         const int s = kb % kStages;
@@ -108,7 +135,6 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
     return;
   }
 
-  // ===================== consumers: warpgroup c owns rows 64 c .. 64 c + 63 =====================
   const int c = wg - 1;
   const int t = threadIdx.x & 127;
   float acc[BN / 2];
@@ -129,22 +155,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
   }
   wgmma_wait<0>();
 
-  // ===================== epilogue =====================
   const int warp = t >> 5, lane = t & 31;
   const int rl0 = c * 64 + warp * 16 + (lane >> 2);  // tile rows of acc[.. 0/1] and (+8) acc[.. 2/3]
-  const bf16* gate_vec[2] = {nullptr, nullptr};
-  if (ACT == 2 && ep.gate_row >= 0) {
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const long long grow = (long long)m0 + rl0 + 8 * h;
-      if (grow < M) {
-        const long long bt = grow / ep.S;
-        const int bb = int(bt / ep.T);
-        const int sel = (ep.x_mask != nullptr && ep.x_mask[bt] == 0) ? 1 : 0;
-        gate_vec[h] = ep.mod + ((size_t)(sel * ep.B + bb) * 6 + ep.gate_row) * N;
-      }
-    }
-  }
 #pragma unroll
   for (int j = 0; j < BN / 8; ++j) {
     const int col = j * 8 + 2 * (lane & 3);  // column inside the tile
@@ -159,27 +171,22 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
         x0 = gelu_tanh_f(rbf(x0));
         x1 = gelu_tanh_f(rbf(x1));
       }
-      if (ACT == 3) {
-        x0 = gelu_erf_f(rbf(x0));
-        x1 = gelu_erf_f(rbf(x1));
-      }
-      if (ACT == 2) {
-        const long long grow = (long long)m0 + row;
-        if (grow < M && gcol < N) {
-          float y0 = rbf(x0), y1 = rbf(x1);  // the Linear's 16-bit output
-          if (gate_vec[h] != nullptr) {
-            const float2 g = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(gate_vec[h] + gcol)));
-            y0 = rbf(g.x * y0);  // bf16(gate * y)
-            y1 = rbf(g.y * y1);
-          }
-          const float2 xr = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(ep.resid + (size_t)grow * N + gcol));
-          x0 = xr.x + y0;  // residual add (rounded by the pack below)
-          x1 = xr.y + y1;
-        }
-      }
-      // 128B swizzle of the staging chunk: conflict-free (the 8 rows of a store land in 8 different 16-byte units)
       unsigned char* dst = smem_c + (col >> 6) * (kBM * 128) + row * 128 + ((((col & 63) >> 3) ^ (row & 7)) << 4) + (col & 7) * 2;
-      *reinterpret_cast<uint32_t*>(dst) = pack_bf16x2(x0, x1);
+      *reinterpret_cast<uint32_t*>(dst) = pack_bf16x2(x0, x1);  // ACT 3: the rounded pre-activation, see below
+    }
+  }
+  if (ACT == 3) {
+    // erf-GELU in a second pass over the thread's own staging slots, once the accumulators are dead: erff next to the
+    // live accumulators would not fit in the register budget.  The slot holds rbf(x), the value the GELU is evaluated
+    // on; the empty asm makes the compiler reload it rather than carry the first pass's registers over.
+    asm volatile("" ::: "memory");
+#pragma unroll
+    for (int i = 0; i < BN / 4; ++i) {
+      const int col = (i >> 1) * 8 + 2 * (lane & 3), row = rl0 + 8 * (i & 1);
+      uint32_t* dst = reinterpret_cast<uint32_t*>(smem_c + (col >> 6) * (kBM * 128) + row * 128 +
+                                                  ((((col & 63) >> 3) ^ (row & 7)) << 4) + (col & 7) * 2);
+      const float2 v = unpack_bf16x2(*dst);
+      *dst = pack_bf16x2(gelu_erf_f(v.x), gelu_erf_f(v.y));
     }
   }
   fence_proxy_async_smem();
@@ -194,35 +201,275 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
 }
 
 template <int BN, int ACT>
-static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tw, const CUtensorMap& tc, const bf16* bias, int M,
-                       int N, int K, cudaStream_t st, const EpiArgs& ep) {
-  using Cfg = GemmCfg<BN>;
+static int launch_gemm_tile(const void* A, const void* W, const bf16* bias, void* out, int M, int N, int K,
+                            const CUtensorMap& ta, cudaStream_t st) {
   static bool attr = false;
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_wgmma_kernel<BN, ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg::kSmemBytes);
+    cudaError_t e = cudaFuncSetAttribute(gemm_tile_kernel<BN, ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         TileCfg<BN>::kSmemBytes);
     if (e != cudaSuccess) return fail(VSB_ERR_CUDA, "gemm: smem attr: %s", cudaGetErrorString(e));
     attr = true;
   }
-  const int tiles = ((M + kBM - 1) / kBM) * ((N + BN - 1) / BN);
-  gemm_wgmma_kernel<BN, ACT><<<tiles, kGemmThreads, Cfg::kSmemBytes, st>>>(ta, tw, tc, bias, M, N, K, ep);
+  CUtensorMap tw, tc;
+  unsigned long long dw[2] = {(unsigned long long)K, (unsigned long long)N};
+  unsigned long long sw[1] = {(unsigned long long)K * 2};
+  unsigned bw[2] = {kBK, (unsigned)BN};
+  int rc = make_tmap_bf16(&tw, W, 2, dw, sw, bw, CU_TENSOR_MAP_SWIZZLE_128B);
+  if (rc) return rc;
+  unsigned long long dc[2] = {(unsigned long long)N, (unsigned long long)M};
+  unsigned long long sc[1] = {(unsigned long long)N * 2};
+  unsigned bc[2] = {64, kBM};
+  rc = make_tmap_bf16(&tc, out, 2, dc, sc, bc, CU_TENSOR_MAP_SWIZZLE_128B);
+  if (rc) return rc;
+  const long long tiles = (long long)((M + kBM - 1) / kBM) * ((N + BN - 1) / BN);
+  gemm_tile_kernel<BN, ACT><<<(unsigned)tiles, kTileThreads, TileCfg<BN>::kSmemBytes, st>>>(ta, tw, tc, bias, M, N, K);
+  return check_launch("gemm_tile");
+}
+
+// ---- persistent ping-pong kernel: the epilogues that cost (gate + residual, GELU at short K) ------------------------
+// TMA store from a 32-bit shared-memory address (the consumers keep no 64-bit pointer live across the mainloop)
+__device__ __forceinline__ void tma_store_2d_s(const CUtensorMap* m, uint32_t src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(reinterpret_cast<uint64_t>(m)),
+               "r"(src), "r"(c0), "r"(c1)
+               : "memory");
+}
+
+template <int ACT>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_w,
+                  const __grid_constant__ CUtensorMap tm_c, const __grid_constant__ CUtensorMap tm_r,
+                  const bf16* __restrict__ bias, int M, int N, int K, const EpiArgs ep) {
+  using Cfg = GemmCfg;
+  constexpr int kStages = Cfg::kStages;
+  extern __shared__ unsigned char smem_dyn[];
+  unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~uintptr_t(1023));
+  unsigned char* smem_ab = smem;                              // [kStages][A 16 KB | W 16 KB]
+  unsigned char* smem_c = smem + kStages * Cfg::kStageBytes;  // [consumer][kBN/64][128 rows][128 B] swizzled
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem_c + 2 * Cfg::kCBytes);  // [kStages]
+  uint64_t* empty = full + kStages;                                         // [kStages]
+  uint64_t* c_full = empty + kStages;   // [2] resid block landed in the consumer's staging tile (ACT 2)
+  uint64_t* c_empty = c_full + 2;       // [2] the consumer's last TMA store has read its staging tile (ACT 2)
+
+  const int wg = threadIdx.x >> 7;
+  const int tiles_n = (N + kBN - 1) / kBN;
+  const int tiles = ((M + kBM - 1) / kBM) * tiles_n;
+  const int num_kb = (K + kBK - 1) / kBK;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tm_a);
+    tma_prefetch_desc(&tm_w);
+    tma_prefetch_desc(&tm_c);
+    if (ACT == 2) tma_prefetch_desc(&tm_r);
+    for (int i = 0; i < kStages; ++i) {
+      mbar_init(&full[i], 1);
+      mbar_init(&empty[i], 1);  // each stage is read by the one consumer that owns its tile
+    }
+    for (int i = 0; i < 2; ++i) {
+      mbar_init(&c_full[i], 1);
+      mbar_init(&c_empty[i], 1);
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (wg == 2) {
+    // ===================== TMA producer =====================
+    if (threadIdx.x == 256) {
+      int n = 0;  // k-blocks loaded so far: the position in the ring, carried over between tiles
+      int j = 0;  // tile of this CTA; consumer j & 1 owns it
+      for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x, ++j) {
+        const int m0 = (tile / tiles_n) * kBM, n0 = (tile % tiles_n) * kBN;
+        for (int kb = 0; kb < num_kb; ++kb, ++n) {
+          const int s = n % kStages;
+          mbar_wait_quiet(&empty[s], ((n / kStages) & 1) ^ 1);
+          unsigned char* sa = smem_ab + s * Cfg::kStageBytes;
+          mbar_arrive_expect_tx(&full[s], Cfg::kStageBytes);
+          tma_load_2d(&tm_a, &full[s], sa, kb * kBK, m0);
+          tma_load_2d(&tm_w, &full[s], sa + Cfg::kABytes, kb * kBK, n0);
+          if (ACT == 2 && kb == min(kStages, num_kb) - 1) {
+            // the resid block, once the ring holds the tile's first k-blocks: the consumer is done with its previous
+            // tile's staging by the time it needs more of this tile's k-blocks
+            const int c = j & 1, u = j >> 1;  // u: the consumer's tile count so far
+            if (u > 0) mbar_wait_quiet(&c_empty[c], (u - 1) & 1);
+            const int nch = min(kBN / 64, (N - n0 + 63) / 64);  // 64-column chunks inside N
+            unsigned char* dst = smem_c + c * Cfg::kCBytes;
+            mbar_arrive_expect_tx(&c_full[c], nch * kBM * 128);
+            for (int ch = 0; ch < nch; ++ch) tma_load_2d(&tm_r, &c_full[c], dst + ch * (kBM * 128), n0 + ch * 64, m0);
+          }
+        }
+      }
+    }
+    return;
+  }
+
+  // ===================== consumers: warpgroup c takes the CTA's tiles j = c, c + 2, ... =====================
+  const int c = wg;
+  const int t = threadIdx.x & 127;
+  const int warp = t >> 5, lane = t & 31;
+  const uint32_t my_c = smem_u32(smem_c) + c * Cfg::kCBytes;
+  const uint32_t ab0 = smem_u32(smem_ab);
+  int u = 0;  // this consumer's tiles so far
+  for (int j = c, tile = blockIdx.x + c * gridDim.x; tile < tiles; j += 2, tile += 2 * gridDim.x, ++u) {
+    const int m0 = (tile / tiles_n) * kBM, n0 = (tile % tiles_n) * kBN;
+    float acc[2][64];
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int i = 0; i < 64; ++i) acc[h][i] = 0.f;
+
+    if (j > 0) named_bar_sync(1 + c, 256);  // our turn: the other consumer has issued its mainloop of tile j - 1
+    const int n_base = j * num_kb;          // ring position of this tile's first k-block
+    for (int kb = 0; kb < num_kb; ++kb) {
+      const int n = n_base + kb, s = n % kStages;
+      mbar_wait_quiet(&full[s], (n / kStages) & 1);
+      const uint32_t sa = ab0 + s * Cfg::kStageBytes;
+      const uint32_t sw = sa + Cfg::kABytes;
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kBK / 16; ++k) {
+        const uint64_t dw = wgmma_desc_sw128(sw + 32 * k);
+        wgmma_m64n128k16_ss(acc[0], wgmma_desc_sw128(sa + 32 * k), dw, 1u);
+        wgmma_m64n128k16_ss(acc[1], wgmma_desc_sw128(sa + 64 * 128 + 32 * k), dw, 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();  // the group of k-block kb - 1 has retired: its stage can be refilled
+      if (kb > 0 && t == 0) mbar_arrive(&empty[(n - 1) % kStages]);
+    }
+    if (tile + gridDim.x < tiles) named_bar_arrive(1 + (c ^ 1), 256);  // hand the tensor cores to tile j + 1
+    wgmma_wait<0>();
+    if (t == 0) mbar_arrive(&empty[(n_base + num_kb - 1) % kStages]);
+
+    // ===================== epilogue =====================
+    // thread rows: rl + 8 h + 64 hm for acc[hm][.. 2 h / 2 h + 1].  Every row of a thread has the same row % 8, so the
+    // 128B swizzle of the staging chunk is one XOR per 8-column group: conflict-free (the 8 rows of a store land in 8
+    // different 16-byte units).
+    const int rl = warp * 16 + (lane >> 2);
+    const uint32_t c_row = my_c + rl * 128 + (lane & 3) * 4;
+    int gate_off[2][2] = {{-1, -1}, {-1, -1}};  // element offset of the row's gate vector in mod, -1: none
+    if (ACT == 2 && ep.gate_row >= 0) {
+#pragma unroll
+      for (int hm = 0; hm < 2; ++hm)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int grow = m0 + rl + 8 * h + 64 * hm;
+          if (grow < M) {
+            const int bt = grow / ep.S;
+            const int bb = bt / ep.T;
+            const int sel = (ep.x_mask != nullptr && ep.x_mask[bt] == 0) ? 1 : 0;
+            gate_off[hm][h] = ((sel * ep.B + bb) * 6 + ep.gate_row) * N;
+          }
+        }
+    }
+    if (ACT == 2) mbar_wait_quiet(&c_full[c], u & 1);  // the resid block is in the staging tile
+#pragma unroll
+    for (int jj = 0; jj < kBN / 8; ++jj) {
+      const int col = jj * 8 + 2 * (lane & 3);  // column inside the tile
+      const int gcol = n0 + col;
+      float2 b2 = make_float2(0.f, 0.f);
+      if (bias != nullptr && gcol < N) b2 = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(bias + gcol)));
+#pragma unroll
+      for (int hm = 0; hm < 2; ++hm)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = rl + 8 * h + 64 * hm;
+          float x0 = acc[hm][4 * jj + 2 * h] + b2.x, x1 = acc[hm][4 * jj + 2 * h + 1] + b2.y;
+          const uint32_t dst = c_row + (jj >> 3) * (kBM * 128) + (8 * h + 64 * hm) * 128 + (((jj & 7) ^ (rl & 7)) << 4);
+          if (ACT == 1) {
+            x0 = gelu_tanh_f(rbf(x0));
+            x1 = gelu_tanh_f(rbf(x1));
+          }
+          if (ACT == 2) {
+            if (m0 + row < M && gcol < N) {
+              float y0 = rbf(x0), y1 = rbf(x1);  // the Linear's 16-bit output
+              if (gate_off[hm][h] >= 0) {
+                const float2 g = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(ep.mod + gate_off[hm][h] + gcol)));
+                y0 = rbf(g.x * y0);  // bf16(gate * y)
+                y1 = rbf(g.y * y1);
+              }
+              uint32_t r;
+              asm volatile("ld.shared.b32 %0, [%1];" : "=r"(r) : "r"(dst));  // resid, landed by TMA in the same slot
+              const float2 xr = unpack_bf16x2(r);
+              x0 = xr.x + y0;  // residual add (rounded by the pack below)
+              x1 = xr.y + y1;
+            }
+          }
+          asm volatile("st.shared.b32 [%0], %1;" ::"r"(dst), "r"(pack_bf16x2(x0, x1)) : "memory");  // ACT 3: rbf(x)
+        }
+    }
+    if (ACT == 3) {
+      // erf-GELU in a second pass over the thread's own staging slots (as in gemm_tile_kernel)
+#pragma unroll 8
+      for (int i = 0; i < kBN / 2; ++i) {
+        const int jj = i >> 2, hm = (i >> 1) & 1, h = i & 1;
+        const uint32_t dst = c_row + (jj >> 3) * (kBM * 128) + (8 * h + 64 * hm) * 128 + (((jj & 7) ^ (rl & 7)) << 4);
+        uint32_t r;
+        asm volatile("ld.shared.b32 %0, [%1];" : "=r"(r) : "r"(dst));
+        const float2 v = unpack_bf16x2(r);
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(dst), "r"(pack_bf16x2(gelu_erf_f(v.x), gelu_erf_f(v.y))) : "memory");
+      }
+    }
+    fence_proxy_async_smem();
+    named_bar_sync(3 + c, 128);
+    if (t == 0) {
+#pragma unroll 1
+      for (int ch = 0; ch < kBN / 64; ++ch)
+        if (n0 + ch * 64 < N) tma_store_2d_s(&tm_c, my_c + ch * (kBM * 128), n0 + ch * 64, m0);
+      tma_store_commit();
+      // the staging tile is rewritten by this consumer's next tile, after the turn barrier above (or the resid load
+      // the producer issues on c_empty): wait here, under the other consumer's mainloop, until the store has read it
+      tma_store_wait_read0();
+      if (ACT == 2) mbar_arrive(&c_empty[c]);
+    }
+  }
+  if (t == 0) tma_store_wait0();
+}
+
+template <int ACT>
+static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tw, const CUtensorMap& tc, const CUtensorMap& tr,
+                       const bf16* bias, int M, int N, int K, cudaStream_t st, const EpiArgs& ep) {
+  static bool attr = false;
+  if (!attr) {
+    cudaError_t e = cudaFuncSetAttribute(gemm_wgmma_kernel<ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         GemmCfg::kSmemBytes);
+    if (e != cudaSuccess) return fail(VSB_ERR_CUDA, "gemm: smem attr: %s", cudaGetErrorString(e));
+    attr = true;
+  }
+  const long long tiles = (long long)((M + kBM - 1) / kBM) * ((N + kBN - 1) / kBN);
+  const int grid = tiles < num_sms() ? int(tiles) : num_sms();
+  gemm_wgmma_kernel<ACT><<<grid, kGemmThreads, GemmCfg::kSmemBytes, st>>>(ta, tw, tc, tr, bias, M, N, K, ep);
   return check_launch("gemm_wgmma");
 }
 
 // act: 0 none, 1 tanh-GELU, 2 fused residual (ep->resid != nullptr), 3 erf-GELU
 static int gemm_dispatch(const void* A, const void* W, const void* bias, void* out, int M, int N, int K, int act,
                          cudaStream_t st, const EpiArgs& ep) {
-  // tile width: 192 divides every STDiT3 / CogVideoX / Latte width (1152, 1920, 2304, 3072, 3456, 4608, 7680); narrow
-  // outputs and widths that 128 divides but 192 does not take 128
-  const int BN = (N % 192 == 0 || (N > 192 && N % 128 != 0)) ? 192 : 128;
-  CUtensorMap ta, tw, tc;
+  if ((long long)((M + kBM - 1) / kBM) * ((N + kBN - 1) / kBN) > 0x7fffffffLL)
+    return fail(VSB_ERR_UNSUPPORTED, "gemm: too many tiles (M=%d N=%d)", M, N);
+  CUtensorMap ta, tw, tc, tr;
   unsigned long long da[2] = {(unsigned long long)K, (unsigned long long)M};
   unsigned long long sa[1] = {(unsigned long long)K * 2};
   unsigned ba[2] = {kBK, kBM};
   int rc = make_tmap_bf16(&ta, A, 2, da, sa, ba, CU_TENSOR_MAP_SWIZZLE_128B);
   if (rc) return rc;
+  const bf16* b = (const bf16*)bias;
+  // The persistent kernel's K loop is slower than the one-tile-per-CTA kernel's (0.671 against 0.521 ms per 1152 of K at
+  // N 1152, H100 SXM, DESIGN.md section 9); what it saves per tile is the fill, the store and the epilogue.  The gate +
+  // residual epilogue saves more than the K loop costs at every K measured (up to 4608); a bias-only epilogue never does;
+  // a GELU epilogue only while K is short.
+  if (act == 0 || ((act == 1 || act == 3) && K > kPersistentGeluMaxK)) {
+    // tile width: 192 divides every STDiT3 / CogVideoX / Latte width (1152, 1920, 2304, 3072, 3456, 4608, 7680); narrow
+    // outputs and widths that 128 divides but 192 does not take 128
+    const bool wide = N % 192 == 0 || (N > 192 && N % 128 != 0);
+#define VSB_TILE_CASE(a)                                                                                      \
+  if (act == a) return wide ? launch_gemm_tile<192, a>(A, W, b, out, M, N, K, ta, st)                         \
+                            : launch_gemm_tile<128, a>(A, W, b, out, M, N, K, ta, st);
+    VSB_TILE_CASE(0)
+    VSB_TILE_CASE(1)
+    VSB_TILE_CASE(3)
+#undef VSB_TILE_CASE
+  }
   unsigned long long dw[2] = {(unsigned long long)K, (unsigned long long)N};
-  unsigned bw[2] = {kBK, (unsigned)BN};
+  unsigned bw[2] = {kBK, (unsigned)kBN};
   rc = make_tmap_bf16(&tw, W, 2, dw, sa, bw, CU_TENSOR_MAP_SWIZZLE_128B);
   if (rc) return rc;
   unsigned long long dc[2] = {(unsigned long long)N, (unsigned long long)M};
@@ -230,18 +477,15 @@ static int gemm_dispatch(const void* A, const void* W, const void* bias, void* o
   unsigned bc[2] = {64, kBM};
   rc = make_tmap_bf16(&tc, out, 2, dc, sc, bc, CU_TENSOR_MAP_SWIZZLE_128B);
   if (rc) return rc;
-  const bf16* b = (const bf16*)bias;
-#define VSB_GEMM_CASE(bn)                                                     \
-  if (BN == bn) {                                                             \
-    if (act == 3) return launch_gemm<bn, 3>(ta, tw, tc, b, M, N, K, st, ep);  \
-    if (act == 2) return launch_gemm<bn, 2>(ta, tw, tc, b, M, N, K, st, ep);  \
-    if (act == 1) return launch_gemm<bn, 1>(ta, tw, tc, b, M, N, K, st, ep);  \
-    return launch_gemm<bn, 0>(ta, tw, tc, b, M, N, K, st, ep);                \
+  if (act == 2) {
+    rc = make_tmap_bf16(&tr, ep.resid, 2, dc, sc, bc, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (rc) return rc;
+  } else {
+    tr = tc;  // unused
   }
-  VSB_GEMM_CASE(192)
-  VSB_GEMM_CASE(128)
-#undef VSB_GEMM_CASE
-  return fail(VSB_ERR_UNSUPPORTED, "gemm: no tile config");
+  if (act == 3) return launch_gemm<3>(ta, tw, tc, tr, b, M, N, K, st, ep);
+  if (act == 2) return launch_gemm<2>(ta, tw, tc, tr, b, M, N, K, st, ep);
+  return launch_gemm<1>(ta, tw, tc, tr, b, M, N, K, st, ep);
 }
 
 }  // namespace vsb
