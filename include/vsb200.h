@@ -263,8 +263,9 @@ int vsb_ipc_close_handle(void* devptr);
  *   zero padded.  out = bf16(conv + bias) [+ resid, rounded again: the ResNet sum of :298]; round_conv = 1 rounds the
  *   convolution to 16 bits before the bias is added.  Cin = 16 or a multiple of 64; Cout = 3 or a multiple of 64.
  * vsb_vae_groupnorm_stats: mean and rstd = rsqrt(var + eps) (fp32, stats [B, G, 2]) of nn.GroupNorm over x [B, P, C]
- *   (P = T*H*W pixels).  workspace: B * VSB_GN_CHUNKS * C * 2 floats.  Fixed-order reduction, no atomics: repeated
- *   launches are bit-identical.  C in {64, 128, 256, 512}, G | C.
+ *   (P = T*H*W pixels).  workspace: B * VSB_GN_CHUNKS * C * 2 floats.  The sums are shifted by each channel's value at
+ *   the sample's first pixel, so a DC offset large against the spread does not cancel the variance away.  Fixed-order
+ *   reduction, no atomics: repeated launches are bit-identical.  C in {64, 128, 256, 512}, G | C.
  * vsb_vae_spatial_norm_silu: silu(GroupNorm(f) * conv_y(zq) + conv_b(zq)) (CogVideoXSpatialNorm3D :165-178, then the
  *   ResNet's nonlinearity :280,:291 or conv_act :867), each eager op rounded.  zyb [B, Tz, h, w, 2C] holds conv_y | conv_b
  *   at latent resolution, gathered with F.interpolate's nearest rule (the odd frame count split of :166-174).  The result

@@ -178,6 +178,9 @@ int launch_conv(const CUtensorMap& tx, const CUtensorMap& tw, const ConvArgs& a,
 // ---------------------------------------------------------------------------------------------------------------------
 // GroupNorm statistics: kGnChunks CTAs per sample each sum a fixed pixel subset per channel (fp32), then one thread per
 // (sample, group) adds the partials in a fixed order in fp64.  No atomics: repeated launches are bit-identical.
+// The sums are of x - k and (x - k)^2 with a pivot k per (sample, channel), the sample's first pixel: on a DC offset
+// large against the spread (a flat region of a frame) plain E[x^2] - mean^2 in fp32 loses the variance to cancellation.
+// The finalize merges the channels' (mean, M2) into the group's in fp64 (Chan et al.).
 // ---------------------------------------------------------------------------------------------------------------------
 constexpr int kGnThreads = 256;
 
@@ -187,20 +190,31 @@ __global__ void __launch_bounds__(kGnThreads) gn_partial_kernel(const bf16* __re
   const int tpp = C / 8, ppi = kGnThreads / tpp;  // threads per pixel, pixels per iteration
   const int v = threadIdx.x % tpp, pl = threadIdx.x / tpp;
   const int b = blockIdx.y, chunk = blockIdx.x;
-  float s[8], q[8];
+  float s[8], q[8], k[8];
+  const bf16* xb = x + (size_t)b * P * C;
+  {
+    const uint4 u = __ldg(reinterpret_cast<const uint4*>(xb + v * 8));
+    const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const float2 f = unpack_bf16x2(w[i]);
+      k[2 * i] = f.x;
+      k[2 * i + 1] = f.y;
+    }
+  }
 #pragma unroll
   for (int i = 0; i < 8; ++i) s[i] = q[i] = 0.f;
-  const bf16* xb = x + (size_t)b * P * C;
   for (long long p = (long long)chunk * ppi + pl; p < P; p += (long long)VSB_GN_CHUNKS * ppi) {
     const uint4 u = __ldg(reinterpret_cast<const uint4*>(xb + p * C + v * 8));
     const uint32_t w[4] = {u.x, u.y, u.z, u.w};
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       const float2 f = unpack_bf16x2(w[i]);
-      s[2 * i] += f.x;
-      s[2 * i + 1] += f.y;
-      q[2 * i] = fmaf(f.x, f.x, q[2 * i]);
-      q[2 * i + 1] = fmaf(f.y, f.y, q[2 * i + 1]);
+      const float d0 = f.x - k[2 * i], d1 = f.y - k[2 * i + 1];
+      s[2 * i] += d0;
+      s[2 * i + 1] += d1;
+      q[2 * i] = fmaf(d0, d0, q[2 * i]);
+      q[2 * i + 1] = fmaf(d1, d1, q[2 * i + 1]);
     }
   }
 #pragma unroll
@@ -222,22 +236,36 @@ __global__ void __launch_bounds__(kGnThreads) gn_partial_kernel(const bf16* __re
   }
 }
 
-__global__ void gn_finalize_kernel(const float* __restrict__ part, float* __restrict__ stats, long long P, int C, int G,
-                                   int B, float eps) {
+// one channel's pivot-shifted sums over all chunks, in fp64: s = sum(x - k), q = sum((x - k)^2)
+__device__ __forceinline__ void gn_channel_sums(const float* __restrict__ part, int b, int c, int C, double& s, double& q) {
+  s = q = 0.0;
+  for (int k = 0; k < VSB_GN_CHUNKS; ++k) {
+    const float* pk = part + ((size_t)b * VSB_GN_CHUNKS + k) * C * 2 + 2 * c;
+    s += pk[0];
+    q += pk[1];
+  }
+}
+
+__global__ void gn_finalize_kernel(const bf16* __restrict__ x, const float* __restrict__ part, float* __restrict__ stats,
+                                   long long P, int C, int G, int B, float eps) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= B * G) return;
   const int b = i / G, g = i % G, cg = C / G;
-  double s = 0.0, q = 0.0;
-  for (int k = 0; k < VSB_GN_CHUNKS; ++k) {
-    const float* pk = part + ((size_t)b * VSB_GN_CHUNKS + k) * C * 2 + 2 * g * cg;
-    for (int c = 0; c < cg; ++c) {
-      s += pk[2 * c];
-      q += pk[2 * c + 1];
-    }
+  const bf16* pivot = x + (size_t)b * P * C + (size_t)g * cg;
+  const double np = (double)P;
+  double s, q, msum = 0.0;
+  for (int c = 0; c < cg; ++c) {
+    gn_channel_sums(part, b, g * cg + c, C, s, q);
+    msum += (double)e_to_float(pivot[c]) + s / np;
   }
-  const double n = (double)P * cg;
-  const double mean = s / n;
-  const double var = fmax(q / n - mean * mean, 0.0);
+  const double mean = msum / cg;
+  double m2 = 0.0;  // sum over the group of (x - mean)^2: each channel's M2 plus its mean's offset from the group's
+  for (int c = 0; c < cg; ++c) {
+    gn_channel_sums(part, b, g * cg + c, C, s, q);
+    const double dm = (double)e_to_float(pivot[c]) + s / np - mean;
+    m2 += fmax(q - s * s / np, 0.0) + np * dm * dm;
+  }
+  const double var = m2 / (np * cg);
   stats[2 * i] = (float)mean;
   stats[2 * i + 1] = rsqrtf((float)var + eps);
 }
@@ -394,7 +422,7 @@ extern "C" int VSB_API(vsb_vae_groupnorm_stats)(const vsb_bf16* x, float* stats,
   gn_partial_kernel<<<dim3(VSB_GN_CHUNKS, B), kGnThreads, 0, st>>>((const bf16*)x, workspace, P, C);
   int rc = check_launch("vae_groupnorm_stats");
   if (rc) return rc;
-  gn_finalize_kernel<<<(B * G + 127) / 128, 128, 0, st>>>(workspace, stats, P, C, G, B, eps);
+  gn_finalize_kernel<<<(B * G + 127) / 128, 128, 0, st>>>((const bf16*)x, workspace, stats, P, C, G, B, eps);
   return check_launch("vae_groupnorm_stats");
 }
 
