@@ -261,7 +261,8 @@ int vsb_ipc_close_handle(void* devptr);
  *   padding (:131-132) is not materialised.  w_packed [Cout_pad, kt*9, Cin_pad] is the weight packed tap-major (tap =
  *   (dt*3 + dy)*3 + dx), Cin_pad / Cout_pad = Cin / Cout rounded up to a multiple of 64,
  *   zero padded.  out = bf16(conv + bias) [+ resid, rounded again: the ResNet sum of :298]; round_conv = 1 rounds the
- *   convolution to 16 bits before the bias is added.  Cin = 16 or a multiple of 64; Cout = 3 or a multiple of 64.
+ *   convolution to 16 bits before the bias is added.  Cin = 16 or a multiple of 64; Cout = 3, 4 or a multiple of 64
+ *   (4: the OpenSora v1.2 temporal decoder's conv_out).
  * vsb_vae_groupnorm_stats: mean and rstd = rsqrt(var + eps) (fp32, stats [B, G, 2]) of nn.GroupNorm over x [B, P, C]
  *   (P = T*H*W pixels).  workspace: B * VSB_GN_CHUNKS * C * 2 floats.  The sums are shifted by each channel's value at
  *   the sample's first pixel, so a DC offset large against the spread does not cancel the variance away.  Fixed-order
@@ -288,7 +289,9 @@ int vsb_vae_upsample2x(const vsb_bf16* x, vsb_bf16* out, int B, int T, int H, in
  *
  * vsb_vae_groupnorm_act: Normalize = nn.GroupNorm(G, C, eps=1e-6) of x (stats from vsb_vae_groupnorm_stats, kept in the
  *   16-bit dtype as torch does), then with act = 1 the nonlinearity x * torch.sigmoid(x) (v1.2.0 :100-101, v1.1.0
- *   :1255-1256), each eager op rounded.  Writes frames t_off .. t_off+T-1 of out [B, T_out, H, W, C].  C % 8 == 0, G | C.
+ *   :1255-1256), each eager op rounded, or with act = 2 F.silu (nn.SiLU of the OpenSora v1.2 temporal and spatial
+ *   decoders): x / (1 + exp(-x)) in fp32, rounded once.  Writes frames t_off .. t_off+T-1 of out [B, T_out, H, W, C].
+ *   C % 8 == 0, G | C.
  * vsb_vae_upsample_linear2x: F.interpolate(mode="trilinear", align_corners=False) of x [B, T, H, W, C] by 2 in H and W
  *   (spatial) and by 2 in T over frames 1.. with frame 0 kept (temporal; Spatial2xTime2x3DUpsample v1.2.0 :349-357,
  *   TimeUpsample2x / TimeUpsampleRes2x v1.1.0 :1549-1596), fp32, rounded once.  To = 1 + 2 (T - 1) frames when temporal
@@ -313,6 +316,15 @@ int vsb_vae_attn_split(const vsb_bf16* qkv, vsb_bf16* q, vsb_bf16* k, vsb_bf16* 
                        int mixed, void* stream);
 int vsb_vae_attn_softmax(vsb_bf16* S, int rows, int P, int Pp, float scale, void* stream);
 int vsb_vae_attn_merge(const vsb_bf16* o, vsb_bf16* out, int B, int T, int P, int C, void* stream);
+
+/* ---- OpenSora v1.2 VAE decoder (models/autoencoders/autoencoder_kl_open_sora.py) ------------------------------------
+ * The temporal decoder and the SDXL image decoder run on the entries above (vsb_vae_groupnorm_act with act = 2,
+ * vsb_vae_conv3d with Cout = 4, the attention split / softmax and the GEMM) plus:
+ * vsb_vae_depth_to_time: rearrange "B (C ts) T H W -> B C (T ts) H W" with ts = 2 on channels-last tensors: channel
+ *   2c + ts of frame t of x [B, T, H, W, 2C] is channel c of frame t_off + 2t + ts of out [B, T_out, H, W, C].  Pure data
+ *   movement (bit exact).  C % 8 == 0, 16-byte aligned pointers. */
+int vsb_vae_depth_to_time(const vsb_bf16* x, vsb_bf16* out, int B, int T, int H, int W, int C, int t_off, int T_out,
+                          void* stream);
 
 /* ---- IEEE fp16 twins ----------------------------------------------------------------------------------------------
  * The reference runs CogVideoX-2b and Latte in torch.float16 (pipelines/cogvideox/pipeline_cogvideox.py:138-139,
@@ -385,6 +397,8 @@ int vsb_vae_attn_split_f16(const vsb_f16* qkv, vsb_f16* q, vsb_f16* k, vsb_f16* 
                            int mixed, void* stream);
 int vsb_vae_attn_softmax_f16(vsb_f16* S, int rows, int P, int Pp, float scale, void* stream);
 int vsb_vae_attn_merge_f16(const vsb_f16* o, vsb_f16* out, int B, int T, int P, int C, void* stream);
+int vsb_vae_depth_to_time_f16(const vsb_f16* x, vsb_f16* out, int B, int T, int H, int W, int C, int t_off, int T_out,
+                              void* stream);
 
 #ifdef __cplusplus
 }

@@ -12,7 +12,8 @@
 //                   tap-major packed weights [Cout_pad, taps * Cin_pad].
 //   warpgroups 1-2  consumers: pixel rows 0..63 / 64..127, wgmma.m64nBNk16 from the swizzled stages.
 //   epilogue        + bias (rounded the way torch's convolution rounds, see round_conv), optional + residual, masked
-//                   stores of the valid pixels and the Cout real channels (Cout = 3 for conv_out).
+//                   stores of the valid pixels and the Cout real channels (Cout = 3 for conv_out, 4 for the OpenSora
+//                   temporal decoder's).
 #include "vsb_common.cuh"
 #include "vsb_host.h"
 #include "wgmma.cuh"
@@ -386,7 +387,8 @@ extern "C" int VSB_API(vsb_vae_conv3d)(const vsb_bf16* x, const vsb_bf16* w_pack
     return fail(VSB_ERR_INVALID, "vae_conv3d: bad args");
   if (kt != 1 && kt != 3) return fail(VSB_ERR_UNSUPPORTED, "vae_conv3d: kt=%d (need 1 or 3)", kt);
   if (!(Cin == 16 || Cin % 64 == 0)) return fail(VSB_ERR_UNSUPPORTED, "vae_conv3d: Cin=%d (need 16 or a multiple of 64)", Cin);
-  if (!(Cout == 3 || Cout % 64 == 0)) return fail(VSB_ERR_UNSUPPORTED, "vae_conv3d: Cout=%d (need 3 or a multiple of 64)", Cout);
+  if (!(Cout == 3 || Cout == 4 || Cout % 64 == 0))
+    return fail(VSB_ERR_UNSUPPORTED, "vae_conv3d: Cout=%d (need 3, 4 or a multiple of 64)", Cout);
   if (!aligned16(x) || !aligned16(w_packed) || (resid && ((uintptr_t)resid & 3)) || ((uintptr_t)out & 3))
     return fail(VSB_ERR_UNSUPPORTED, "vae_conv3d: misaligned pointer");
   const int BN = Cout % 128 == 0 ? 128 : 64;

@@ -2,7 +2,9 @@
 // vae_conv.cu does not already provide.  Activations are channels-last [B, T, H, W, C] 16-bit tensors throughout.
 //
 //   groupnorm_act_kernel    nn.GroupNorm(32, C, eps=1e-6) with the statistics of vsb_vae_groupnorm_stats, optionally followed
-//                           by the reference's nonlinearity x * torch.sigmoid(x) (two eager ops, each rounded)
+//                           by the reference's nonlinearity x * torch.sigmoid(x) (two eager ops, each rounded) or by
+//                           F.silu (one rounding; nn.SiLU of the OpenSora v1.2 decoders)
+//   depth_to_time_kernel    OpenSora's temporal decoder: [B, T, H, W, 2C] -> [B, 2T, H, W, C], a 16-byte gather copy
 //   upsample_linear_kernel  F.interpolate(mode="trilinear", align_corners=False) by 2 in H and W and / or in T over frames
 //                           1.. (Spatial2xTime2x3DUpsample, TimeUpsample2x, TimeUpsampleRes2x)
 //   mix_kernel              TimeUpsampleRes2x's alpha * x + (1 - alpha) * conv(x), each eager op rounded
@@ -64,7 +66,10 @@ __global__ void __launch_bounds__(256) groupnorm_act_kernel(const GnArgs a) {
         const float sc = rstd * (e ? gg.y : gg.x);
         const float sh = fmaf(-sc, mean, e ? bb.y : bb.x);
         const float n = rbf(fmaf(sc, e ? xx.y : xx.x, sh));
-        r[e] = a.act ? n * rbf(1.f / (1.f + expf(-n))) : n;
+        if (a.act == 2)
+          r[e] = n / (1.f + expf(-n));  // F.silu: x / (1 + exp(-x)) in fp32, rounded once
+        else
+          r[e] = a.act ? n * rbf(1.f / (1.f + expf(-n))) : n;
       }
       o[k] = pack_bf16x2(r[0], r[1]);
     }
@@ -255,11 +260,51 @@ __global__ void __launch_bounds__(256) attn_merge_kernel(const bf16* __restrict_
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Depth to time (OpenSora's temporal decoder, rearrange "B (C ts) T H W -> B C (T ts) H W", ts = 2): channel 2c + ts of
+// input frame t is channel c of output frame 2t + ts.  One thread per 16 input channels of a pixel: two 16-byte loads,
+// the even / odd halves of each 32-bit word sorted apart, one 16-byte store into each of the two output frames.
+// ---------------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) depth_to_time_kernel(const bf16* __restrict__ x, bf16* __restrict__ out, int B, int T,
+                                                            int HW, int C, int t_off, int T_out) {
+  const int nv = C / 8;  // output vectors per pixel = input vectors per pixel / 2
+  const long long total = (long long)B * T * HW * nv;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int v = (int)(i % nv);
+    long long p = i / nv;
+    const int px = (int)(p % HW);
+    p /= HW;
+    const int t = (int)(p % T), b = (int)(p / T);
+    const uint4* src = reinterpret_cast<const uint4*>(x + (size_t)i * 16);
+    const uint4 u0 = __ldg(src), u1 = __ldg(src + 1);
+    const uint32_t w[8] = {u0.x, u0.y, u0.z, u0.w, u1.x, u1.y, u1.z, u1.w};
+    uint32_t ev[4], od[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      ev[k] = __byte_perm(w[2 * k], w[2 * k + 1], 0x5410);  // low halves: ts = 0
+      od[k] = __byte_perm(w[2 * k], w[2 * k + 1], 0x7632);  // high halves: ts = 1
+    }
+    const size_t o0 = (((size_t)b * T_out + t_off + 2 * t) * HW + px) * C + v * 8;
+    *reinterpret_cast<uint4*>(out + o0) = make_uint4(ev[0], ev[1], ev[2], ev[3]);
+    *reinterpret_cast<uint4*>(out + o0 + (size_t)HW * C) = make_uint4(od[0], od[1], od[2], od[3]);
+  }
+}
+
 }  // namespace
 
 }  // namespace vsb
 
 using namespace vsb;
+
+extern "C" int VSB_API(vsb_vae_depth_to_time)(const vsb_bf16* x, vsb_bf16* out, int B, int T, int H, int W, int C, int t_off,
+                                              int T_out, void* stream) {
+  if (!x || !out || B <= 0 || T <= 0 || H <= 0 || W <= 0 || C <= 0 || t_off < 0 || t_off + 2 * T > T_out)
+    return fail(VSB_ERR_INVALID, "vae_depth_to_time: bad args");
+  if (C % 8 || !aligned16(x) || !aligned16(out)) return fail(VSB_ERR_UNSUPPORTED, "vae_depth_to_time: need C %% 8 == 0, 16B-aligned");
+  depth_to_time_kernel<<<grid_for((long long)B * T * H * W * (C / 8)), 256, 0, (cudaStream_t)stream>>>((const bf16*)x, (bf16*)out, B, T,
+                                                                                                       H * W, C, t_off, T_out);
+  return check_launch("vae_depth_to_time");
+}
 
 extern "C" int VSB_API(vsb_vae_groupnorm_act)(const vsb_bf16* x, const float* stats, const vsb_bf16* gamma, const vsb_bf16* beta,
                                               vsb_bf16* out, int B, int T, int H, int W, int C, int G, int t_off, int T_out,
@@ -270,7 +315,8 @@ extern "C" int VSB_API(vsb_vae_groupnorm_act)(const vsb_bf16* x, const float* st
   if (C % 8 || C % G) return fail(VSB_ERR_UNSUPPORTED, "vae_groupnorm_act: C=%d G=%d", C, G);
   if (!aligned16(x) || !aligned16(gamma) || !aligned16(beta) || !aligned16(out))
     return fail(VSB_ERR_UNSUPPORTED, "vae_groupnorm_act: misaligned pointer");
-  GnArgs a{(const bf16*)x, stats, (const bf16*)gamma, (const bf16*)beta, (bf16*)out, B, T, H * W, C, G, t_off, T_out, act ? 1 : 0};
+  GnArgs a{(const bf16*)x, stats, (const bf16*)gamma, (const bf16*)beta, (bf16*)out, B, T, H * W, C, G, t_off, T_out,
+           act == 2 ? 2 : (act ? 1 : 0)};
   groupnorm_act_kernel<<<grid_for((long long)B * T * H * W * (C / 8)), 256, 0, (cudaStream_t)stream>>>(a);
   return check_launch("vae_groupnorm_act");
 }

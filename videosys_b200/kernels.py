@@ -331,8 +331,9 @@ def vae_upsample2x(x, compress_time):
 
 
 def vae_groupnorm_act(x, stats, gamma, beta, out=None, t_off=0, act=True):
-    """GroupNorm of x [B, T, H, W, C] with stats from vae_groupnorm_stats, then x * sigmoid(x) when act, into frames
-    t_off .. t_off+T-1 of out [B, T_out, H, W, C] (default: a new [B, T, H, W, C])."""
+    """GroupNorm of x [B, T, H, W, C] with stats from vae_groupnorm_stats, then x * sigmoid(x) when act is true (1),
+    F.silu (one rounding) when act == 2, into frames t_off .. t_off+T-1 of out [B, T_out, H, W, C] (default: a new
+    [B, T, H, W, C])."""
     lib, st = _prep(x, stats, gamma, beta, out)
     _bf16(x, "x")
     _same_dtype(x, gamma, beta, out)
@@ -340,7 +341,23 @@ def vae_groupnorm_act(x, stats, gamma, beta, out=None, t_off=0, act=True):
     out = torch.empty_like(x) if out is None else out
     with _Timed("vae_groupnorm_act", 2 * x.numel() * 2):
         _lib.check(_fn(lib, "vsb_vae_groupnorm_act", x)(_p(x), _p(stats), _p(gamma), _p(beta), _p(out), B, T, H, W, C, stats.shape[1],
-                                                        t_off, out.shape[1], int(bool(act)), st), "vae_groupnorm_act")
+                                                        t_off, out.shape[1], 2 if act == 2 else int(bool(act)), st), "vae_groupnorm_act")
+    return out
+
+
+def vae_depth_to_time(x, out=None, t_off=0):
+    """rearrange "B (C ts) T H W -> B C (T ts) H W" (ts = 2) of x [B, T, H, W, 2C] into frames t_off .. t_off+2T-1 of out
+    [B, T_out, H, W, C] (default: a new [B, 2T, H, W, C])."""
+    lib, st = _prep(x, out)
+    _bf16(x, "x")
+    _same_dtype(x, out)
+    B, T, H, W, C2 = x.shape
+    if C2 % 2:
+        raise _lib.VsbError(f"vae_depth_to_time: odd channel count {C2}")
+    out = torch.empty(B, 2 * T, H, W, C2 // 2, dtype=x.dtype, device=x.device) if out is None else out
+    with _Timed("vae_depth_to_time", 2 * x.numel() * 2):
+        _lib.check(_fn(lib, "vsb_vae_depth_to_time", x)(_p(x), _p(out), B, T, H, W, C2 // 2, t_off, out.shape[1], st),
+                   "vae_depth_to_time")
     return out
 
 

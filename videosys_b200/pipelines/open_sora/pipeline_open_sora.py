@@ -1,10 +1,16 @@
 """OpenSora pipeline surface (mirror of videosys/pipelines/open_sora/pipeline_open_sora.py: OpenSoraPABConfig :32-69,
 OpenSoraConfig :126-163, OpenSoraPipeline.generate :426-656) around the native STDiT3.
 
-In scope: the config classes, ``generate()``'s signature, the shape tables, the RFLOW loop and the denoiser.
-Out of scope (SURVEY.md 2.1 rows 7, 9): the T5 text encoder, prompt cleaning and the VAE decode -- they run once per
-video, not per step.  ``text_encoder`` / ``vae`` may be passed as callables; without them ``generate`` feeds a
-deterministic synthetic caption embedding and returns the denoised LATENTS (the quantity the metric is defined on).
+In scope: the config classes, ``generate()``'s signature, the shape tables, the RFLOW loop and the denoiser, and the VAE
+decode on the native OpenSora v1.2 decoder (models/autoencoders/autoencoder_kl_open_sora.py).  Out of scope (SURVEY.md 2.1
+row 7): the T5 text encoder and prompt cleaning -- pass a ``text_encoder_fn``; without it ``generate`` feeds a
+deterministic synthetic caption embedding.
+
+The decode is opt-in: ``OpenSoraConfig(vae=<local snapshot directory or VideoAutoencoderPipeline instance>)`` makes
+``generate`` return the reference's uint8 video ``[B, T, H, W, 3]`` (:638-648).  The default ``vae`` is the hub id
+"hpcai-tech/OpenSora-VAE-v1.2", which is not a local directory, so by default ``generate`` returns the denoised LATENTS
+exactly as before (the quantity the metric is defined on).  A ``vae_decode_fn`` takes precedence over both.  Under
+sequence parallelism every rank decodes the whole video, as the reference does.
 """
 import zlib
 from dataclasses import dataclass
@@ -74,6 +80,8 @@ class OpenSoraConfig:
                  transformer_config: Optional[STDiT3Config] = None, state_dict=None,
                  text_encoder_fn: Optional[Callable] = None, vae_decode_fn: Optional[Callable] = None):
         self.pipeline_cls = OpenSoraPipeline
+        # vae: a local snapshot directory of hpcai-tech/OpenSora-VAE-v1.2 or a VideoAutoencoderPipeline instance decodes
+        # natively; anything else (the default hub id) leaves generate() returning latents
         self.transformer, self.vae, self.text_encoder = transformer, vae, text_encoder
         self.num_gpus = num_gpus
         self.num_sampling_steps = num_sampling_steps
@@ -114,9 +122,28 @@ class OpenSoraPipeline:
         self.transformer = self.transformer.to(self._device).eval()
         self.scheduler = RFLOW(num_sampling_steps=config.num_sampling_steps, cfg_scale=config.cfg_scale,
                                use_timestep_transform=True)
+        self.vae = self._load_vae()
         if config.enable_pab:
             set_pab_manager(config.pab_config)
         self._set_parallel()
+
+    def _load_vae(self):
+        """The native VAE of ``config.vae`` in bf16 on the pipeline's device (the reference builds it with
+        micro_batch_size = config.tiling_size, :215-220), or None when ``config.vae`` is not a local directory or an
+        instance."""
+        from ...models.autoencoders.autoencoder_kl_open_sora import load_vae
+
+        vae = load_vae(self._config.vae, micro_batch_size=self._config.tiling_size)
+        return None if vae is None else vae.to(torch.bfloat16).to(self._device).eval()
+
+    def decode_latents(self, samples, num_frames: int):
+        """The reference tail (:638-648): vae(samples, decode_only=True, num_frames), then clamp_(-1, 1), sub_(-1),
+        div_(2), mul(255), add_(0.5), clamp_(0, 255) in bf16, as uint8 [B, T, H, W, 3] on the CPU."""
+        video = self.vae.decode(samples.to(torch.bfloat16), num_frames=num_frames)
+        low, high = -1, 1
+        video.clamp_(min=low, max=high)
+        video.sub_(low).div_(max(high - low, 1e-5))
+        return video.mul(255).add_(0.5).clamp_(0, 255).permute(0, 2, 3, 4, 1).to("cpu", torch.uint8)
 
     def _set_parallel(self, dp_size=None, sp_size=None, enable_cp=False):
         import torch.distributed as dist
@@ -194,6 +221,8 @@ class OpenSoraPipeline:
         samples = self.scheduler.sample(self.transformer, z, margs, y_null.to(dev, dtype), dev, mask=masks, progress=verbose)
         if self._config.vae_decode_fn is not None:
             video = self._config.vae_decode_fn(samples, nf)
+        elif getattr(self, "vae", None) is not None:
+            video = self.decode_latents(samples, nf)
         else:
-            video = samples.float().cpu()  # latents: the VAE is out of scope
+            video = samples.float().cpu()  # latents: no local VAE
         return VideoSysPipelineOutput(video=video) if return_dict else (video,)
