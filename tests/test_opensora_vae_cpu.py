@@ -1,6 +1,6 @@
 """OpenSora v1.2 VAE decoder: the host logic (micro-frame chunks, time padding and trim, zero causal context, the
 depth-to-time shuffle, latent padding, image micro-batches, weight packing) on the torch stand-ins of the kernels
-(tests/kernels_emul_opensora_vae.py), fp32, against the outputs of the UNMODIFIED reference decode in
+(tests/kernels_emul_vae.py), fp32, against the outputs of the UNMODIFIED reference decode in
 tests/golden/opensora_vae.pt (oracle/gen_golden_opensora_vae.py); the state-dict layout against the reference and the
 restated SDXL decoder; snapshot loading; and the pipeline's decode stage."""
 import os
@@ -10,7 +10,7 @@ import torch
 
 from oracle import ref_loader
 from oracle.gen_golden_opensora_vae import CASES, NARROW, latents, sample_index, weights
-from tests import kernels_emul_opensora_vae
+from tests import kernels_emul_vae
 from videosys_b200.models.autoencoders import VideoAutoencoderPipeline
 
 
@@ -27,7 +27,7 @@ def _vae(name, **kw):
 
 @pytest.mark.parametrize("name", list(CASES))
 def test_opensora_vae_decode_vs_reference_golden(monkeypatch, gold, name):
-    kernels_emul_opensora_vae.emulate(monkeypatch)
+    kernels_emul_vae.emulate(monkeypatch)
     out = _vae(name).decode(latents(name), num_frames=CASES[name][2])
     assert list(out.shape) == gold[f"{name}.shape"]
     flat = out.flatten()
@@ -38,7 +38,7 @@ def test_opensora_vae_decode_vs_reference_golden(monkeypatch, gold, name):
 
 def test_opensora_vae_micro_batches_do_not_change_the_result(monkeypatch):
     """Each image is its own GroupNorm sample: one spatial pass per frame or all frames at once decode alike."""
-    kernels_emul_opensora_vae.emulate(monkeypatch)
+    kernels_emul_vae.emulate(monkeypatch)
     a = _vae("batch2", micro_batch_size=1).decode(latents("batch2"), num_frames=17)
     b = _vae("batch2", micro_batch_size=None).decode(latents("batch2"), num_frames=17)
     assert torch.allclose(a, b, rtol=1e-5, atol=1e-5)
@@ -171,7 +171,7 @@ def _reference_tail(vae, samples, num_frames):
 
 
 def test_opensora_generate_with_native_vae_instance_and_dir(monkeypatch, tmp_path):
-    kernels_emul_opensora_vae.emulate(monkeypatch)
+    kernels_emul_vae.emulate(monkeypatch)
     vae = _vae("one_chunk")
     pipe, _ = _pipeline(vae)
     pipe.vae = pipe._load_vae()
@@ -192,7 +192,7 @@ def test_opensora_generate_with_native_vae_instance_and_dir(monkeypatch, tmp_pat
 
 
 def test_opensora_generate_default_config_returns_latents(monkeypatch):
-    kernels_emul_opensora_vae.emulate(monkeypatch)
+    kernels_emul_vae.emulate(monkeypatch)
     pipe, P = _pipeline(None)
     assert pipe._config.vae == "hpcai-tech/OpenSora-VAE-v1.2"
     pipe.vae = pipe._load_vae()
@@ -203,7 +203,7 @@ def test_opensora_generate_default_config_returns_latents(monkeypatch):
 
 
 def test_opensora_generate_vae_decode_fn_takes_precedence(monkeypatch):
-    kernels_emul_opensora_vae.emulate(monkeypatch)
+    kernels_emul_vae.emulate(monkeypatch)
     calls = []
     pipe, _ = _pipeline(_vae("image"), vae_decode_fn=lambda s, nf: calls.append((tuple(s.shape), nf)) or "decoded")
     pipe.vae = pipe._load_vae()

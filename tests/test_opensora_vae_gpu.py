@@ -8,7 +8,7 @@ import pytest
 import torch
 
 from oracle.gen_golden_opensora_vae import CASES, NARROW, latents, sample_index, weights
-from tests import kernels_emul_opensora_vae as EOS
+from tests import kernels_emul_vae as EV
 from tests import vae_fp64 as V
 from videosys_b200 import kernels
 from videosys_b200.models.autoencoders import VideoAutoencoderPipeline
@@ -91,7 +91,7 @@ def test_vae_conv3d_cout4_zero_context_fp64(name, dtype):
 @pytest.mark.parametrize("B,T,H,W,C", [(1, 5, 90, 160, 512), (2, 3, 5, 7, 256), (1, 1, 1, 1, 8)])
 def test_vae_depth_to_time_bit_exact(B, T, H, W, C, dtype):
     x = _act(B, T, H, W, 2 * C, dtype=dtype, seed=7)
-    want = EOS.vae_depth_to_time(x)  # the reference's einops rearrange
+    want = EV.vae_depth_to_time(x)  # the reference's einops rearrange
     V.assert_bit_exact(f"depth_to_time B={B} T={T} {H}x{W} C={C} {dtype}", kernels.vae_depth_to_time(x), want)
     buf = torch.full((B, 2 * T + 3, H, W, C), float("nan"), dtype=dtype, device=DEV)
     kernels.vae_depth_to_time(x, out=buf, t_off=2)
@@ -114,7 +114,7 @@ def _vae(name, dtype=torch.bfloat16):
 def _eager(monkeypatch, vae, z, nf):
     """The eager torch / cuDNN decoder: the same module on the kernels' stand-ins."""
     with monkeypatch.context() as m:
-        for n, f in EOS.stand_ins().items():
+        for n, f in EV.stand_ins().items():
             m.setattr(kernels, n, f)
         return vae.decode(z, num_frames=nf)
 

@@ -1,6 +1,6 @@
 """Open-Sora-Plan causal-VAE decoder (v1.1.0 and v1.2.0): the host logic (context buffers, latent padding, attention
 layouts, up-samplers, tiling and blending, weight packing) on the torch stand-ins of the kernels
-(tests/kernels_emul_osp_vae.py), fp32, against the outputs of the UNMODIFIED reference decoders in tests/golden/osp_vae.pt
+(tests/kernels_emul_vae.py), fp32, against the outputs of the UNMODIFIED reference decoders in tests/golden/osp_vae.pt
 (oracle/gen_golden_osp_vae.py); the state-dict layout against the reference; checkpoint loading; the rejections; and the
 pipeline's decode stage."""
 import json
@@ -11,7 +11,7 @@ import torch
 
 from oracle import ref_loader
 from oracle.gen_golden_osp_vae import CASES, V110_RES, V120, apply_tiling, latents, sample_index, weights
-from tests import kernels_emul_osp_vae
+from tests import kernels_emul_vae
 from videosys_b200.models.autoencoders import CausalVAEModelV110, CausalVAEModelV120
 from videosys_b200.models.autoencoders.autoencoder_kl_open_sora_plan import decoder_class
 
@@ -40,13 +40,13 @@ def _check(out, gold, name):
 
 @pytest.mark.parametrize("name", list(CASES))
 def test_osp_vae_decode_vs_reference_golden(monkeypatch, gold, name):
-    kernels_emul_osp_vae.emulate(monkeypatch)
+    kernels_emul_vae.emulate(monkeypatch)
     _check(_vae(name).decode(latents(name)), gold, name)
 
 
 def test_osp_vae_tiled_case_really_tiles(monkeypatch):
     """The tiled golden case runs several time chunks and overlapping tiles; untiled it decodes to the same shape."""
-    kernels_emul_osp_vae.emulate(monkeypatch)
+    kernels_emul_vae.emulate(monkeypatch)
     vae = _vae("v110_tiled")
     calls = []
     orig = vae._decode_tile
@@ -183,7 +183,7 @@ def _generate(pipe, output_type="pil"):
 
 
 def test_osp_generate_with_native_vae_matches_reference_tail(monkeypatch):
-    kernels_emul_osp_vae.emulate(monkeypatch)
+    kernels_emul_vae.emulate(monkeypatch)
     vae = _vae("v110_default_f3")
     pipe = _pipeline(monkeypatch, vae)
     video = _generate(pipe)
@@ -195,7 +195,7 @@ def test_osp_generate_with_native_vae_matches_reference_tail(monkeypatch):
 
 
 def test_osp_generate_without_vae_returns_the_same_latents(monkeypatch):
-    kernels_emul_osp_vae.emulate(monkeypatch)
+    kernels_emul_vae.emulate(monkeypatch)
     with_vae = _generate(_pipeline(monkeypatch, _vae("v110_default_f3")), "latents")
     pipe = _pipeline(monkeypatch, None)
     assert pipe.vae is None
@@ -205,7 +205,7 @@ def test_osp_generate_without_vae_returns_the_same_latents(monkeypatch):
 
 
 def test_osp_pipeline_applies_the_reference_tiling(monkeypatch, tmp_path):
-    kernels_emul_osp_vae.emulate(monkeypatch)
+    kernels_emul_vae.emulate(monkeypatch)
     pipe = _pipeline(monkeypatch, _vae("v110_default_f3"), enable_tiling=True)
     v = pipe.vae
     assert v.use_tiling and (v.tile_sample_min_size, v.tile_latent_min_size, v.tile_sample_min_size_t, v.tile_latent_min_size_t) == \

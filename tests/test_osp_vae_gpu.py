@@ -10,10 +10,9 @@ import torch
 import torch.nn.functional as F
 
 from oracle.gen_golden_osp_vae import CASES, apply_tiling, latents, sample_index, weights
-from tests import kernels_emul as E
-from tests import kernels_emul_osp_vae as EO
 from tests import kernels_emul_vae as EV
 from videosys_b200 import kernels
+from videosys_b200.models.autoencoders._common import frame_attention
 from videosys_b200.models.autoencoders.autoencoder_kl_open_sora_plan import decoder_class
 
 pytestmark = pytest.mark.gpu
@@ -76,44 +75,19 @@ def test_vae_groupnorm_act_vs_eager(name, act, dtype):
 ATTN_SHAPES = {"fix_60x80_t1": (1, 60, 80, False), "attn3d_64x64_t2": (2, 64, 64, True)}
 
 
-def _eager_attention(qkv, C, mixed):
-    """The reference's bmm / scale / softmax / bmm on the (b*t, c, h*w) views (AttnBlock3D :920-932, Fix :387-411)."""
-    B, T, H, W, _ = qkv.shape
-    q, k, v = (EO._to_reference_frames(qkv[..., i * C:(i + 1) * C], mixed) for i in range(3))
-    w_ = torch.bmm(q.permute(0, 2, 1), k) * (int(C) ** (-0.5))
-    w_ = F.softmax(w_, dim=2)
-    h_ = torch.bmm(v, w_.permute(0, 2, 1))  # (bt, c, hw)
-    if mixed:
-        return h_.reshape(B, C, T, H, W).permute(0, 2, 3, 4, 1)
-    return h_.reshape(B, T, C, H, W).permute(0, 1, 3, 4, 2)
-
-
-def _native_attention(qkv, C, mixed):
-    B, T, H, W, _ = qkv.shape
-    q, k, vt = kernels.vae_attn_split(qkv, C, mixed)
-    P, Pp = H * W, k.shape[1]
-    o = torch.empty(B * T, P, C, dtype=qkv.dtype, device=DEV)
-    s = torch.empty(P, Pp, dtype=qkv.dtype, device=DEV)
-    for f in range(B * T):
-        kernels.gemm_bias_act(q[f], k[f], out=s)
-        kernels.vae_attn_softmax_(s, P, int(C) ** (-0.5))
-        kernels.gemm_bias_act(s, vt[f], out=o[f])
-    return kernels.vae_attn_merge(o, B, T, H, W) if mixed else o.view(B, T, H, W, C)
-
-
 @pytest.mark.parametrize("dtype", DTYPES, ids=["bf16", "fp16"])
 @pytest.mark.parametrize("name", list(ATTN_SHAPES))
 def test_vae_attention_vs_eager(name, dtype, no_tf32):
     T, H, W, mixed = ATTN_SHAPES[name]
     C = 512
     qkv = _rand(1, T, H, W, 3 * C, dtype=dtype, scale=1.5, seed=4)
-    ours = _native_attention(qkv, C, mixed)
-    eager = _eager_attention(qkv, C, mixed)
-    ref = _eager_attention(qkv.float(), C, mixed).double()
+    ours = frame_attention(qkv, C, mixed)
+    eager = EV.eager_attention(qkv, C, mixed)
+    ref = EV.eager_attention(qkv.float(), C, mixed).double()
     _report(f"attention {name} {dtype}", ours, eager)
     e_ours, e_eager = float((ours.double() - ref).norm()), float((eager.double() - ref).norm())
     print(f"[attention {name} {dtype}] |ours - fp32| = {e_ours:.4g}, |eager16 - fp32| = {e_eager:.4g}, ratio {e_ours / e_eager:.3f}")
-    assert torch.equal(ours, _native_attention(qkv, C, mixed))
+    assert torch.equal(ours, frame_attention(qkv, C, mixed))
     assert e_ours <= 1.25 * e_eager
 
 
@@ -140,7 +114,7 @@ LIN_SHAPES = {"spatial_time_256_120x160_t3": (3, 120, 160, 256, True, True), "sp
 def test_vae_upsample_linear2x_vs_interpolate(name, dtype):
     T, H, W, C, sp, tm = LIN_SHAPES[name]
     x = _rand(1, T, H, W, C, dtype=dtype, seed=6)
-    want = EO.vae_upsample_linear2x(x, sp, tm)  # F.interpolate trilinear, as the reference calls it
+    want = EV.vae_upsample_linear2x(x, sp, tm)  # F.interpolate trilinear, as the reference calls it
     To = want.shape[1]
     buf = torch.empty(1, To + 2, *want.shape[2:], dtype=dtype, device=DEV)
     got = kernels.vae_upsample_linear2x(x, sp, tm, out=buf, t_off=2)[:, 2:]
@@ -173,9 +147,8 @@ def _vae(name, dtype):
 def _eager(monkeypatch, vae, z):
     """The eager torch / cuDNN decoder: the same module on the kernels' stand-ins."""
     with monkeypatch.context() as m:
-        for mod, names in ((EV, EV.NAMES), (EO, EO.NAMES), (E, ["gemm_bias_act", "gemm_bias_residual"])):
-            for n in names:
-                m.setattr(kernels, n, getattr(mod, n))
+        for n, f in EV.stand_ins().items():
+            m.setattr(kernels, n, f)
         return vae.decode(z)
 
 

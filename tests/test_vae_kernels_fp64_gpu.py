@@ -9,11 +9,10 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from tests import kernels_emul_osp_vae as EO
 from tests import kernels_emul_vae as EV
 from tests import vae_fp64 as V
-from tests.test_osp_vae_gpu import _eager_attention, _native_attention
 from videosys_b200 import kernels
+from videosys_b200.models.autoencoders._common import frame_attention
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -240,7 +239,7 @@ def test_vae_attn_split_merge_bit_exact(mixed, C, T, dtype):
     for H, W in ((3, 5), (10, 10), (60, 80)):
         qkv = _act(B, T, H, W, 3 * C, dtype=dtype, seed=40 + H)
         q, k, vt = kernels.vae_attn_split(qkv, C, mixed)
-        rq, rk, rvt = EO.vae_attn_split(qkv, C, mixed)  # torch reshape / permute, zero padded
+        rq, rk, rvt = EV.vae_attn_split(qkv, C, mixed)  # torch reshape / permute, zero padded
         what = f"attn_split mixed={int(mixed)} C={C} T={T} P={H * W} {dtype}"
         V.assert_bit_exact(what + " q", q, rq)
         V.assert_bit_exact(what + " k", k, rk)
@@ -291,9 +290,9 @@ def test_vae_attention_path_fp64(name, dtype, monkeypatch):
     monkeypatch.setattr(torch.backends.cuda.matmul, "allow_tf32", False)
     T, H, W, C, mixed = ATTN_CASES[name]
     qkv = _rand(2, T, H, W, 3 * C, dtype=dtype, scale=1.5, seed=70)
-    ours = _native_attention(qkv, C, mixed)
-    eager = _eager_attention(qkv, C, mixed)
-    exact = _eager_attention(qkv.double(), C, mixed)
+    ours = frame_attention(qkv, C, mixed)
+    eager = EV.eager_attention(qkv, C, mixed)
+    exact = EV.eager_attention(qkv.double(), C, mixed)
     err, err_eager = (ours.double() - exact).abs(), (eager.double() - exact).abs()
     print(f"[attention {name} {dtype}] max|err| vs fp64 {float(err.max()):.3e} (eager16 {float(err_eager.max()):.3e}), "
           f"mean {float(err.mean()):.3e} (eager16 {float(err_eager.mean()):.3e})")
@@ -324,8 +323,8 @@ LIN_CASES = {  # name: (B, T, H, W, C, spatial, temporal)
 def test_vae_upsample_linear2x_fp64(name, dtype):
     B, T, H, W, C, sp, tm = LIN_CASES[name]
     x = _act(B, T, H, W, C, dtype=dtype, seed=80)
-    v = EO.vae_upsample_linear2x(x.double(), sp, tm)  # F.interpolate trilinear in float64, frames 1.. on their own
-    mag = EO.vae_upsample_linear2x(x.double().abs(), sp, tm)  # sum of |weight * tap|
+    v = EV.vae_upsample_linear2x(x.double(), sp, tm)  # F.interpolate trilinear in float64, frames 1.. on their own
+    mag = EV.vae_upsample_linear2x(x.double().abs(), sp, tm)  # sum of |weight * tap|
     To = v.shape[1]
     buf = torch.full((B, To + 3, *v.shape[2:]), float("nan"), dtype=dtype, device=DEV)
     kernels.vae_upsample_linear2x(x, sp, tm, out=buf, t_off=2)
@@ -349,4 +348,4 @@ def test_vae_mix_bit_exact(T, dtype):
     xbuf, y = _act(2, T + 3, 12, 20, 128, dtype=dtype, seed=100), _act(2, T, 12, 20, 128, dtype=dtype, seed=101)
     alpha = torch.sigmoid(torch.tensor([0.7], dtype=dtype, device=DEV))
     a, oma = float(alpha), float(1 - alpha)
-    V.assert_bit_exact(f"mix T={T} {dtype}", kernels.vae_mix(xbuf, y, a, oma, t_off=2), EO.vae_mix(xbuf, y, a, oma, t_off=2))
+    V.assert_bit_exact(f"mix T={T} {dtype}", kernels.vae_mix(xbuf, y, a, oma, t_off=2), EV.vae_mix(xbuf, y, a, oma, t_off=2))

@@ -12,17 +12,13 @@ and shapes under ``decoder.*``.  Activations stay channels-last ``[B, T, H, W, C
   - ``conv_shortcut`` (1x1x1) is a GEMM on the pixel rows; the ResNet sum is the conv2 epilogue.
 The frame batching of ``_decode`` and the tiling of ``tiled_decode`` reproduce the reference's integer arithmetic.
 """
-import inspect
 from typing import Optional, Tuple
 
 import torch
 import torch.nn as nn
 
 from ... import kernels
-
-_GN_CHANNELS = (64, 128, 256, 512)  # channel counts vsb_vae_groupnorm_stats takes
-# torch's GPU convolution (cuDNN) rounds the convolution to 16 bits and adds the bias as a separate op
-ROUND_CONV = True
+from ._common import DecoderOnlyVAE, check_widths, conv_buffer, run_conv, tiled_decode_2d
 
 
 class DecoderOutput:
@@ -40,15 +36,12 @@ class CogVideoXCausalConv3d(nn.Module):
         self.time_kernel_size = kernel_size
         self.conv = nn.Conv3d(in_channels, out_channels, kernel_size)
         self.conv_cache = None
-        self._w = None
 
     def _clear_fake_context_parallel_cache(self):
         self.conv_cache = None
 
     def input_buffer(self, x_shape, dtype, device):
-        """[B, 2 + T, H, W, Cin] for an input of shape [B, T, H, W, Cin]: frames 2.. are the convolution's input."""
-        B, T, H, W, _ = x_shape
-        return torch.empty(B, T + 2, H, W, self.conv.in_channels, dtype=dtype, device=device)
+        return conv_buffer(self.conv, x_shape, dtype, device)
 
     def run(self, buf, resid=None):
         """Fills the two context frames of buf, keeps the new cache, and convolves (reference :123-135)."""
@@ -57,7 +50,7 @@ class CogVideoXCausalConv3d(nn.Module):
         else:
             buf[:, :2] = self.conv_cache
         self.conv_cache = buf[:, -2:].clone()
-        return kernels.vae_conv3d(buf, self._w, self.conv.bias, self.conv.out_channels, 3, resid=resid, round_conv=ROUND_CONV)
+        return run_conv(self.conv, buf, resid)
 
 
 class CogVideoXSpatialNorm3D(nn.Module):
@@ -69,6 +62,10 @@ class CogVideoXSpatialNorm3D(nn.Module):
         self.conv_y = CogVideoXCausalConv3d(zq_channels, f_channels, kernel_size=1)
         self.conv_b = CogVideoXCausalConv3d(zq_channels, f_channels, kernel_size=1)
         self._w = self._b = None
+
+    def pack(self):
+        self._w = torch.cat([self.conv_y.conv.weight, self.conv_b.conv.weight]).flatten(1).detach().contiguous()
+        self._b = torch.cat([self.conv_y.conv.bias, self.conv_b.conv.bias]).detach().contiguous()
 
     def norm_silu_into(self, f, zq, buf):
         """silu(norm(f, zq)) of f [B, T, H, W, C] into frames 2.. of buf; zq [B, Tz, h, w, Cz] is the latent frame batch."""
@@ -96,7 +93,7 @@ class CogVideoXResnetBlock3D(nn.Module):
         buf = self.conv2.input_buffer(h.shape, h.dtype, h.device)
         self.norm2.norm_silu_into(h, zq, buf)
         if self.in_channels != self.out_channels:
-            x = kernels.gemm_bias_act(x, self._w_sc, self.conv_shortcut.bias)
+            x = kernels.gemm_bias_act(x, self.conv_shortcut._w, self.conv_shortcut._b)
         return self.conv2.run(buf, resid=x)
 
 
@@ -107,11 +104,9 @@ class CogVideoXUpsample3D(nn.Module):
         super().__init__()
         self.conv = nn.Conv2d(in_channels, out_channels, kernel_size=3, stride=1, padding=1)
         self.compress_time = compress_time
-        self._w = None
 
     def forward(self, x):
-        u = kernels.vae_upsample2x(x, self.compress_time)
-        return kernels.vae_conv3d(u, self._w, self.conv.bias, self.conv.out_channels, 1, round_conv=ROUND_CONV)
+        return run_conv(self.conv, kernels.vae_upsample2x(x, self.compress_time))
 
 
 class CogVideoXMidBlock3D(nn.Module):
@@ -177,9 +172,9 @@ class CogVideoXDecoder3D(nn.Module):
         return self.conv_out.run(buf).permute(0, 4, 1, 2, 3)
 
 
-class AutoencoderKLCogVideoX(nn.Module):
-    """Reference :872-1239, decoder only.  ``load_state_dict`` takes the reference's full state dict: it drops the
-    ``encoder.*`` and ``quant_conv.*`` entries (the encoder is out of scope) and is strict about every other key."""
+class AutoencoderKLCogVideoX(DecoderOnlyVAE):
+    """Reference :872-1239, decoder only.  ``load_state_dict`` drops the ``encoder.*`` and ``quant_conv.*`` entries of the
+    reference's full state dict."""
 
     _DROPPED_PREFIXES = ("encoder.", "quant_conv.")
 
@@ -201,9 +196,8 @@ class AutoencoderKLCogVideoX(nn.Module):
             raise ValueError("up_block_types and block_out_channels must have the same length")
         if act_fn not in ("silu", "swish"):
             raise ValueError(f"act_fn={act_fn!r}: the decoder kernels apply SiLU")
+        check_widths(block_out_channels, f"block_out_channels {tuple(block_out_channels)}")
         for c in block_out_channels:
-            if c not in _GN_CHANNELS:
-                raise ValueError(f"block_out_channels {tuple(block_out_channels)}: each must be one of {_GN_CHANNELS}")
             if c % norm_num_groups:
                 raise ValueError(f"norm_num_groups={norm_num_groups} does not divide {c} channels")
         if not (latent_channels == 16 or latent_channels % 64 == 0):
@@ -229,22 +223,11 @@ class AutoencoderKLCogVideoX(nn.Module):
         self.tile_latent_min_width = int(self.tile_sample_min_width / (2 ** (len(block_out_channels) - 1)))
         self.tile_overlap_factor_height = 1 / 6
         self.tile_overlap_factor_width = 1 / 5
-        self._pack_key = None
 
     @classmethod
     def from_pretrained(cls, path: str, subfolder: str = "vae"):
         """A LOCAL snapshot directory (``<path>/<subfolder>/config.json`` + weights); no hub download."""
-        from ...utils.checkpoint import load_local_checkpoint
-
-        cfg, sd = load_local_checkpoint(path, subfolder)
-        keys = set(inspect.signature(cls.__init__).parameters) - {"self"}
-        vae = cls(**{k: v for k, v in cfg.items() if k in keys})
-        vae.load_state_dict(sd)
-        return vae
-
-    def load_state_dict(self, state_dict, strict: bool = True):
-        kept = {k: v for k, v in state_dict.items() if not k.startswith(self._DROPPED_PREFIXES)}
-        return super().load_state_dict(kept, strict=strict)
+        return cls._from_local_diffusers(path, subfolder)
 
     @property
     def dtype(self):
@@ -276,98 +259,36 @@ class AutoencoderKLCogVideoX(nn.Module):
     def disable_slicing(self):
         self.use_slicing = False
 
-    def encode(self, x, return_dict: bool = True):
-        raise NotImplementedError("AutoencoderKLCogVideoX.encode: the VAE encoder is out of scope (decoder only)")
-
-    # ---- kernel weights ----
-    def _pack_weights(self):
-        """Packs the convolution weights for the kernels once per set of parameter tensors (after loading, .to(), ...)."""
-        key = tuple((p.data_ptr(), p._version, p.dtype, p.device) for p in self.parameters())
-        if key == self._pack_key:
-            return
-        for m in self.modules():
-            if isinstance(m, CogVideoXCausalConv3d) and m.time_kernel_size == 3:
-                m._w = kernels.pack_conv_weight(m.conv.weight.detach())
-            elif isinstance(m, CogVideoXUpsample3D):
-                m._w = kernels.pack_conv_weight(m.conv.weight.detach())
-            elif isinstance(m, CogVideoXSpatialNorm3D):
-                m._w = torch.cat([m.conv_y.conv.weight, m.conv_b.conv.weight]).flatten(1).detach().contiguous()
-                m._b = torch.cat([m.conv_y.conv.bias, m.conv_b.conv.bias]).detach().contiguous()
-            elif isinstance(m, CogVideoXResnetBlock3D) and m.in_channels != m.out_channels:
-                m._w_sc = m.conv_shortcut.weight.detach().flatten(1).contiguous()
-        self._pack_key = key
-
     # ---- decoding (:1094-1239) ----
+    def _decode_frame_batches(self, z):
+        """The decoder over z's frame batches (the first one takes the remainder), the conv caches carried from batch to
+        batch and cleared after the last."""
+        fbs = self.num_latent_frames_batch_size
+        num_frames = z.shape[2]
+        rem = num_frames % fbs
+        dec = [self.decoder(z[:, :, fbs * i + (0 if i == 0 else rem):fbs * (i + 1) + rem]) for i in range(num_frames // fbs)]
+        self._clear_fake_context_parallel_cache()
+        return torch.cat(dec, dim=2)
+
     def _decode(self, z, return_dict: bool = True):
         batch_size, num_channels, num_frames, height, width = z.shape
         if self.use_tiling and (width > self.tile_latent_min_width or height > self.tile_latent_min_height):
             return self.tiled_decode(z, return_dict=return_dict)
-        fbs = self.num_latent_frames_batch_size
-        dec = []
-        for i in range(num_frames // fbs):
-            rem = num_frames % fbs
-            start, end = fbs * i + (0 if i == 0 else rem), fbs * (i + 1) + rem
-            dec.append(self.decoder(z[:, :, start:end]))
-        self._clear_fake_context_parallel_cache()
-        dec = torch.cat(dec, dim=2)
+        dec = self._decode_frame_batches(z)
         return DecoderOutput(sample=dec) if return_dict else (dec,)
 
     @torch.no_grad()
     def decode(self, z, return_dict: bool = True):
         """z [B, latent_channels, T, h, w] (already divided by scaling_factor) -> [B, out_channels, 4 (T - 1) + 1, 8h, 8w]."""
-        kernels.require_cuda(z, "AutoencoderKLCogVideoX.decode")
-        z = z.to(self.dtype)
-        kernels.require_cuda(z, "AutoencoderKLCogVideoX.decode", half_only=True)
-        self._pack_weights()
+        z = self._decode_input(z)
         if self.use_slicing and z.shape[0] > 1:
             decoded = torch.cat([self._decode(s).sample for s in z.split(1)])
         else:
             decoded = self._decode(z).sample
         return DecoderOutput(sample=decoded) if return_dict else (decoded,)
 
-    def blend_v(self, a, b, blend_extent: int):
-        blend_extent = min(a.shape[3], b.shape[3], blend_extent)
-        for y in range(blend_extent):
-            b[:, :, :, y, :] = a[:, :, :, -blend_extent + y, :] * (1 - y / blend_extent) + b[:, :, :, y, :] * (y / blend_extent)
-        return b
-
-    def blend_h(self, a, b, blend_extent: int):
-        blend_extent = min(a.shape[4], b.shape[4], blend_extent)
-        for x in range(blend_extent):
-            b[:, :, :, :, x] = a[:, :, :, :, -blend_extent + x] * (1 - x / blend_extent) + b[:, :, :, :, x] * (x / blend_extent)
-        return b
-
     def tiled_decode(self, z, return_dict: bool = True):
-        batch_size, num_channels, num_frames, height, width = z.shape
-        overlap_height = int(self.tile_latent_min_height * (1 - self.tile_overlap_factor_height))
-        overlap_width = int(self.tile_latent_min_width * (1 - self.tile_overlap_factor_width))
-        blend_extent_height = int(self.tile_sample_min_height * self.tile_overlap_factor_height)
-        blend_extent_width = int(self.tile_sample_min_width * self.tile_overlap_factor_width)
-        row_limit_height = self.tile_sample_min_height - blend_extent_height
-        row_limit_width = self.tile_sample_min_width - blend_extent_width
-        fbs = self.num_latent_frames_batch_size
-        rows = []
-        for i in range(0, height, overlap_height):
-            row = []
-            for j in range(0, width, overlap_width):
-                time = []
-                for k in range(num_frames // fbs):
-                    rem = num_frames % fbs
-                    start, end = fbs * k + (0 if k == 0 else rem), fbs * (k + 1) + rem
-                    tile = z[:, :, start:end, i:i + self.tile_latent_min_height, j:j + self.tile_latent_min_width]
-                    time.append(self.decoder(tile))
-                self._clear_fake_context_parallel_cache()
-                row.append(torch.cat(time, dim=2))
-            rows.append(row)
-        result_rows = []
-        for i, row in enumerate(rows):
-            result_row = []
-            for j, tile in enumerate(row):
-                if i > 0:
-                    tile = self.blend_v(rows[i - 1][j], tile, blend_extent_height)
-                if j > 0:
-                    tile = self.blend_h(row[j - 1], tile, blend_extent_width)
-                result_row.append(tile[:, :, :, :row_limit_height, :row_limit_width])
-            result_rows.append(torch.cat(result_row, dim=4))
-        dec = torch.cat(result_rows, dim=3)
+        dec = tiled_decode_2d(z, self._decode_frame_batches, (self.tile_latent_min_height, self.tile_latent_min_width),
+                              (self.tile_sample_min_height, self.tile_sample_min_width),
+                              (self.tile_overlap_factor_height, self.tile_overlap_factor_width))
         return DecoderOutput(sample=dec) if return_dict else (dec,)

@@ -28,44 +28,13 @@ import torch
 import torch.nn as nn
 
 from ... import kernels
-from .autoencoder_kl_open_sora_plan import _GN_CHANNELS, _LATENT_PAD
+from ._common import (DecoderOnlyVAE, _cast_tuple, attention, check_widths, conv_buffer, conv_kt, group_norm, pad_1x1,
+                      pad_latent, run_conv)
 
 _SILU = 2  # vae_groupnorm_act's F.silu mode
 SCALE = (3.85, 2.32, 2.33, 3.06)  # OpenSoraVAE_V1_2 (:748-749)
 SHIFT = (-0.10, 0.34, 0.27, 0.98)
 SD_SCALING = 0.18215  # VideoAutoencoderKL.decode divides the latent by this (:534)
-
-
-def _cast_tuple(t, length=1):
-    return tuple(t) if isinstance(t, (tuple, list)) else (t,) * length
-
-
-def _gn(norm, x, out=None, t_off=0, act=_SILU):
-    stats = kernels.vae_groupnorm_stats(x, norm.num_groups, norm.eps)
-    return kernels.vae_groupnorm_act(x, stats, norm.weight, norm.bias, out=out, t_off=t_off, act=act)
-
-
-def _pad_latent(z):
-    """[..., c] (c <= 16) -> [..., 16], zero channels after c: the smallest Cin the convolution and the GEMM take."""
-    zp = torch.zeros(*z.shape[:-1], _LATENT_PAD, dtype=z.dtype, device=z.device)
-    zp[..., :z.shape[-1]] = z
-    return zp
-
-
-def _pad_1x1(weight, bias):
-    """A 4 -> 4 1x1 convolution as a [16, 16] GEMM weight and a [16] bias (zero rows / columns)."""
-    cout, cin = weight.shape[:2]
-    w = torch.zeros(_LATENT_PAD, _LATENT_PAD, dtype=weight.dtype, device=weight.device)
-    w[:cout, :cin] = weight.detach().flatten(1)
-    b = torch.zeros(_LATENT_PAD, dtype=weight.dtype, device=weight.device)
-    b[:cout] = bias.detach()
-    return w, b
-
-
-def _dropped(key: str) -> bool:
-    """Encoder-side keys of the full checkpoint (``*.encoder.*``, ``*.quant_conv.*``): not part of the decoder."""
-    parts = key.split(".")
-    return "encoder" in parts or "quant_conv" in parts
 
 
 # =====================================================================================================================
@@ -76,29 +45,16 @@ class CausalConv3d(nn.Module):
 
     def __init__(self, chan_in, chan_out, kernel_size, bias=True):
         super().__init__()
-        kernel_size = _cast_tuple(kernel_size, 3)
-        self.chan_in, self.chan_out = chan_in, chan_out
-        self.time_kernel_size = kernel_size[0]
-        self.conv = nn.Conv3d(chan_in, chan_out, kernel_size, bias=bias)
-        self._w = self._b = None
-
-    def pack(self):
-        w = self.conv.weight.detach()
-        self._w = kernels.pack_conv_weight(w) if w.shape[-1] == 3 else w.flatten(1).contiguous()
-        b = self.conv.bias
-        self._b = b.detach() if b is not None else torch.zeros(self.chan_out, dtype=w.dtype, device=w.device)
+        self.conv = nn.Conv3d(chan_in, chan_out, _cast_tuple(kernel_size, 3), bias=bias)
 
     def input_buffer(self, x_shape, dtype, device):
-        """[B, kt - 1 + T, H, W, Cin] with the kt - 1 context frames zeroed: frames kt - 1 .. are the caller's."""
-        B, T, H, W, C = x_shape
-        ctx = self.time_kernel_size - 1
-        buf = torch.empty(B, ctx + T, H, W, C, dtype=dtype, device=device)
-        buf[:, :ctx].zero_()
+        """conv_buffer with the kt - 1 context frames zeroed."""
+        buf = conv_buffer(self.conv, x_shape, dtype, device)
+        buf[:, :conv_kt(self.conv) - 1].zero_()
         return buf
 
     def run(self, buf, resid=None):
-        # bias-free convolutions carry a zero bias: bf16(conv + 0) is the rounded convolution
-        return kernels.vae_conv3d(buf, self._w, self._b, self.chan_out, self.time_kernel_size, resid=resid, round_conv=True)
+        return run_conv(self.conv, buf, resid)
 
 
 class ResBlock(nn.Module):
@@ -117,12 +73,12 @@ class ResBlock(nn.Module):
 
     def forward(self, x):
         buf = self.conv1.input_buffer(x.shape, x.dtype, x.device)
-        _gn(self.norm1, x, buf, t_off=2)
+        group_norm(self.norm1, x, buf, t_off=2, act=_SILU)
         h = self.conv1.run(buf)
         buf = self.conv2.input_buffer(h.shape, h.dtype, h.device)
-        _gn(self.norm2, h, buf, t_off=2)
+        group_norm(self.norm2, h, buf, t_off=2, act=_SILU)
         if self.in_channels != self.filters:
-            x = kernels.gemm_bias_act(x, self.conv3._w)
+            x = kernels.gemm_bias_act(x, self.conv3.conv._w)
         return self.conv2.run(buf, resid=x)
 
 
@@ -171,7 +127,7 @@ class Decoder(nn.Module):
                 buf[:, 2:] = x
                 x = kernels.vae_depth_to_time(conv.run(buf))
         buf = self.conv_out.input_buffer(x.shape, x.dtype, x.device)
-        _gn(self.norm1, x, buf, t_off=2)
+        group_norm(self.norm1, x, buf, t_off=2, act=_SILU)
         return self.conv_out.run(buf)
 
 
@@ -189,6 +145,9 @@ class VAE_Temporal(nn.Module):
                                num_res_blocks=num_res_blocks, channel_multipliers=channel_multipliers,
                                temporal_downsample=temporal_downsample, num_groups=num_groups)
         self._pq = None
+
+    def pack(self):
+        self._pq = pad_1x1(self.post_quant_conv.conv.weight, self.post_quant_conv.conv.bias)
 
     def get_latent_size(self, input_size):
         """Reference :424-439."""
@@ -222,16 +181,6 @@ def VAE_Temporal_SD(**kwargs):
 # image decoder: diffusers AutoencoderKL (Decoder, UNetMidBlock2D, UpDecoderBlock2D, ResnetBlock2D, Upsample2D,
 # Attention with AttnProcessor2_0), decoder half, with diffusers' parameter names
 # =====================================================================================================================
-def _conv2d_pack(conv):
-    conv._w = kernels.pack_conv_weight(conv.weight.detach())
-    conv._b = conv.bias.detach()
-
-
-def _conv2d_run(conv, x, resid=None):
-    """A 3x3 Conv2d (padding 1, bias) of x [N, 1, H, W, Cin] -> [N, 1, H, W, Cout]."""
-    return kernels.vae_conv3d(x, conv._w, conv._b, conv.out_channels, 1, resid=resid, round_conv=True)
-
-
 class ResnetBlock2D(nn.Module):
     """norm1 -> SiLU -> conv1 -> norm2 -> SiLU -> conv2, out = (x + h) / 1.0 with x through the 1x1 ``conv_shortcut``
     (bias) where the width changes.  GroupNorm eps 1e-6."""
@@ -247,11 +196,11 @@ class ResnetBlock2D(nn.Module):
             self.conv_shortcut = nn.Conv2d(in_channels, out_channels, 1)
 
     def forward(self, x):
-        h = _conv2d_run(self.conv1, _gn(self.norm1, x))
-        n = _gn(self.norm2, h)
+        h = run_conv(self.conv1, group_norm(self.norm1, x, act=_SILU))
+        n = group_norm(self.norm2, h, act=_SILU)
         if self.in_channels != self.out_channels:
-            x = kernels.gemm_bias_act(x, self.conv_shortcut._w, self.conv_shortcut.bias)
-        return _conv2d_run(self.conv2, n, resid=x)  # dividing by output_scale_factor = 1.0 is exact
+            x = kernels.gemm_bias_act(x, self.conv_shortcut._w, self.conv_shortcut._b)
+        return run_conv(self.conv2, n, resid=x)  # dividing by output_scale_factor = 1.0 is exact
 
 
 class Attention(nn.Module):
@@ -267,19 +216,13 @@ class Attention(nn.Module):
         self.to_out = nn.ModuleList([nn.Linear(channels, channels), nn.Dropout(0.0)])
         self._w_qkv = self._b_qkv = None
 
+    def pack(self):
+        self._w_qkv = torch.cat([self.to_q.weight, self.to_k.weight, self.to_v.weight]).detach().contiguous()
+        self._b_qkv = torch.cat([self.to_q.bias, self.to_k.bias, self.to_v.bias]).detach().contiguous()
+
     def forward(self, x):
-        N, T, H, W, C = x.shape
-        qkv = kernels.gemm_bias_act(_gn(self.group_norm, x, act=False), self._w_qkv, self._b_qkv)
-        q, k, vt = kernels.vae_attn_split(qkv, C, False)
-        P, Pp = H * W, k.shape[1]
-        o = torch.empty(N * T, P, C, dtype=x.dtype, device=x.device)
-        s = torch.empty(P, Pp, dtype=x.dtype, device=x.device)  # one frame's scores at a time
-        for f in range(N * T):
-            kernels.gemm_bias_act(q[f], k[f], out=s)
-            kernels.vae_attn_softmax_(s, P, int(C) ** (-0.5))
-            kernels.gemm_bias_act(s, vt[f], out=o[f])
         out = self.to_out[0]
-        return kernels.gemm_bias_residual(o.view(N, T, H, W, C), out.weight, out.bias, x, out=torch.empty_like(x))
+        return attention(x, self.group_norm, self._w_qkv, self._b_qkv, out.weight, out.bias, False)
 
 
 class UNetMidBlock2D(nn.Module):
@@ -300,7 +243,7 @@ class Upsample2D(nn.Module):
         self.conv = nn.Conv2d(channels, channels, 3, padding=1)
 
     def forward(self, x):
-        return _conv2d_run(self.conv, kernels.vae_upsample2x(x, False))
+        return run_conv(self.conv, kernels.vae_upsample2x(x, False))
 
 
 class UpDecoderBlock2D(nn.Module):
@@ -338,10 +281,10 @@ class SpatialDecoder(nn.Module):
 
     def forward(self, z):
         """z [N, 1, h, w, 16] (frames in the batch, zero padded) -> [N, 1, 8h, 8w, 3]."""
-        x = self.mid_block(_conv2d_run(self.conv_in, z))
+        x = self.mid_block(run_conv(self.conv_in, z))
         for up in self.up_blocks:
             x = up(x)
-        return _conv2d_run(self.conv_out, _gn(self.conv_norm_out, x))
+        return run_conv(self.conv_out, group_norm(self.conv_norm_out, x, act=_SILU))
 
 
 class AutoencoderKL(nn.Module):
@@ -356,6 +299,9 @@ class AutoencoderKL(nn.Module):
         self.post_quant_conv = nn.Conv2d(latent_channels, latent_channels, 1)
         self.decoder = SpatialDecoder(latent_channels, 3, block_out_channels, layers_per_block)
         self._pq = None
+
+    def pack(self):
+        self._pq = pad_1x1(self.post_quant_conv.weight, self.post_quant_conv.bias)
 
     def decode_frames(self, z):
         """z [N, 1, h, w, 16] -> [N, 1, 8h, 8w, 3]."""
@@ -380,14 +326,14 @@ class VideoAutoencoderKL(nn.Module):
         bs = N if self.micro_batch_size is None else self.micro_batch_size
         out = torch.empty(N, 1, 8 * h, 8 * w, 3, dtype=x.dtype, device=x.device)
         for i in range(0, N, bs):
-            out[i:i + bs] = self.module.decode_frames(_pad_latent(x[i:i + bs] / SD_SCALING))
+            out[i:i + bs] = self.module.decode_frames(pad_latent(x[i:i + bs] / SD_SCALING))
         return out.view(B, T, 8 * h, 8 * w, 3)
 
 
 # =====================================================================================================================
 # the pipeline
 # =====================================================================================================================
-class VideoAutoencoderPipeline(nn.Module):
+class VideoAutoencoderPipeline(DecoderOnlyVAE):
     """OpenSora v1.2 VAE (reference :621-729 as built by OpenSoraVAE_V1_2 :731-761), decoder only: ``temporal_vae``
     (VAE_Temporal_SD) and ``spatial_vae.module`` (the SDXL AutoencoderKL), ``scale`` / ``shift`` buffers.
 
@@ -399,10 +345,7 @@ class VideoAutoencoderPipeline(nn.Module):
     def __init__(self, micro_frame_size: Optional[int] = 17, micro_batch_size: Optional[int] = 4,
                  spatial_block_out_channels: Sequence[int] = (128, 256, 512, 512), scale=SCALE, shift=SHIFT):
         super().__init__()
-        bad = [c for c in spatial_block_out_channels if c not in _GN_CHANNELS]
-        if bad or len(spatial_block_out_channels) < 1:
-            raise ValueError(f"spatial_block_out_channels={tuple(spatial_block_out_channels)}: each width must be one of "
-                             f"{_GN_CHANNELS}")
+        check_widths(spatial_block_out_channels, f"spatial_block_out_channels={tuple(spatial_block_out_channels)}")
         self.spatial_vae = VideoAutoencoderKL(micro_batch_size, spatial_block_out_channels)
         self.temporal_vae = VAE_Temporal_SD()
         self.micro_frame_size = micro_frame_size
@@ -411,7 +354,6 @@ class VideoAutoencoderPipeline(nn.Module):
         self.out_channels = self.temporal_vae.out_channels
         self.register_buffer("scale", torch.tensor(scale)[None, :, None, None, None])
         self.register_buffer("shift", torch.tensor(shift)[None, :, None, None, None])
-        self._pack_key = None
 
     # ---- loading ----
     @classmethod
@@ -425,12 +367,14 @@ class VideoAutoencoderPipeline(nn.Module):
         vae.load_state_dict(sd)
         return vae
 
+    def _dropped(self, key: str) -> bool:
+        """Encoder-side keys of the full checkpoint (``*.encoder.*``, ``*.quant_conv.*``): not part of the decoder."""
+        parts = key.split(".")
+        return "encoder" in parts or "quant_conv" in parts
+
     def load_state_dict(self, state_dict, strict: bool = True):
-        kept = {k: v for k, v in state_dict.items() if not _dropped(k)}
-        for k in ("scale", "shift"):
-            if k not in kept:
-                kept[k] = getattr(self, k)
-        return super().load_state_dict(kept, strict=strict)
+        defaults = {k: getattr(self, k) for k in ("scale", "shift") if k not in state_dict}
+        return super().load_state_dict({**state_dict, **defaults}, strict=strict)
 
     @property
     def dtype(self):
@@ -440,47 +384,19 @@ class VideoAutoencoderPipeline(nn.Module):
     def device(self):
         return self.temporal_vae.decoder.norm1.weight.device
 
-    def encode(self, x):
-        raise NotImplementedError(f"{type(self).__name__}.encode: the VAE encoder is out of scope (decoder only)")
-
-    # ---- kernel weights ----
-    def _pack_weights(self):
-        """Packs the weights for the kernels once per set of parameter tensors (after loading, .to(), ...)."""
-        key = tuple((p.data_ptr(), p._version, p.dtype, p.device) for p in self.parameters())
-        if key == self._pack_key:
-            return
-        for m in self.modules():
-            if isinstance(m, CausalConv3d):
-                m.pack()
-            elif isinstance(m, nn.Conv2d) and m.kernel_size == (3, 3):
-                _conv2d_pack(m)
-            elif isinstance(m, nn.Conv2d) and m is not self.spatial_vae.module.post_quant_conv:  # 1x1 conv_shortcut
-                m._w = m.weight.detach().flatten(1).contiguous()
-            elif isinstance(m, Attention):
-                m._w_qkv = torch.cat([m.to_q.weight, m.to_k.weight, m.to_v.weight]).detach().contiguous()
-                m._b_qkv = torch.cat([m.to_q.bias, m.to_k.bias, m.to_v.bias]).detach().contiguous()
-        pq = self.temporal_vae.post_quant_conv.conv
-        self.temporal_vae._pq = _pad_1x1(pq.weight, pq.bias)
-        pq = self.spatial_vae.module.post_quant_conv
-        self.spatial_vae.module._pq = _pad_1x1(pq.weight, pq.bias)
-        self._pack_key = key
-
     # ---- decoding ----
     @torch.no_grad()
     def decode(self, z, num_frames=None):
         """z [B, 4, T, h, w] -> video [B, 3, T', 8h, 8w] in [-1, 1]-ish (reference decode :672-695, cal_loss off)."""
-        kernels.require_cuda(z, f"{type(self).__name__}.decode")
-        z = z.to(self.dtype)
-        kernels.require_cuda(z, f"{type(self).__name__}.decode", half_only=True)
-        self._pack_weights()
+        z = self._decode_input(z)
         z = z * self.scale.to(z.dtype) + self.shift.to(z.dtype)
         zl = z.permute(0, 2, 3, 4, 1)  # [B, T, h, w, 4]
         if self.micro_frame_size is None:
-            x_z = self.temporal_vae.decode(_pad_latent(zl), num_frames=num_frames)
+            x_z = self.temporal_vae.decode(pad_latent(zl), num_frames=num_frames)
         else:
             chunks = []
             for i in range(0, zl.shape[1], self.micro_z_frame_size):
-                z_bs = _pad_latent(zl[:, i:i + self.micro_z_frame_size])
+                z_bs = pad_latent(zl[:, i:i + self.micro_z_frame_size])
                 chunks.append(self.temporal_vae.decode(z_bs, num_frames=min(self.micro_frame_size, num_frames)))
                 num_frames -= self.micro_frame_size
             x_z = torch.cat(chunks, dim=1)

@@ -16,7 +16,6 @@ kernels:
 ``decode``, ``tiled_decode`` and ``tiled_decode2d`` reproduce the reference's integer arithmetic.
 """
 import glob
-import inspect
 import os
 from typing import Optional, Tuple
 
@@ -24,23 +23,13 @@ import torch
 import torch.nn as nn
 
 from ... import kernels
-
-_GN_CHANNELS = (64, 128, 256, 512)  # channel counts vsb_vae_groupnorm_stats takes
-_LATENT_PAD = 16  # latent channels are zero padded to this (the convolution's smallest Cin)
-
-
-def _cast_tuple(t, length=1):
-    return tuple(t) if isinstance(t, (tuple, list)) else (t,) * length
+from ._common import (LATENT_PAD, DecoderOnlyVAE, _cast_tuple, attention, check_widths, conv_buffer, group_norm, pad_1x1,
+                      pad_latent, run_conv, tiled_decode_2d)
 
 
 def _norm(c):
     """Normalize (reference :150-151 / :1179-1180)."""
     return nn.GroupNorm(num_groups=32, num_channels=c, eps=1e-6, affine=True)
-
-
-def _gn(norm, x, out=None, t_off=0, act=True):
-    stats = kernels.vae_groupnorm_stats(x, norm.num_groups, norm.eps)
-    return kernels.vae_groupnorm_act(x, stats, norm.weight, norm.bias, out=out, t_off=t_off, act=act)
 
 
 class CausalConv3d(nn.Module):
@@ -50,30 +39,18 @@ class CausalConv3d(nn.Module):
         super().__init__()
         self.kernel_size = _cast_tuple(kernel_size, 3)
         self.time_kernel_size = self.kernel_size[0]
-        self.chan_in, self.chan_out = chan_in, chan_out
         padding = list(_cast_tuple(padding, 3))
         padding[0] = 0
         self.conv = nn.Conv3d(chan_in, chan_out, self.kernel_size, stride=stride, padding=tuple(padding))
-        self._w = None
-
-    @property
-    def weight(self):
-        return self.conv.weight
-
-    @property
-    def bias(self):
-        return self.conv.bias
 
     def input_buffer(self, x_shape, dtype, device):
-        """[B, kt - 1 + T, H, W, Cin] for an input [B, T, H, W, Cin]: frames kt - 1 .. are the convolution's input."""
-        B, T, H, W, C = x_shape
-        return torch.empty(B, self.time_kernel_size - 1 + T, H, W, C, dtype=dtype, device=device)
+        return conv_buffer(self.conv, x_shape, dtype, device)
 
     def run(self, buf, resid=None):
         kt = self.time_kernel_size
         if kt > 1:
             buf[:, :kt - 1] = buf[:, kt - 1:kt]
-        return kernels.vae_conv3d(buf, self._w, self.bias, self.chan_out, kt, resid=resid, round_conv=True)
+        return run_conv(self.conv, buf, resid)
 
 
 class Conv2d(nn.Conv2d):
@@ -83,11 +60,12 @@ class Conv2d(nn.Conv2d):
 
     def __init__(self, in_channels, out_channels, kernel_size=3, stride=1, padding=0, **kw):
         super().__init__(in_channels, out_channels, kernel_size, stride, padding)
-        self.chan_in, self.chan_out = in_channels, out_channels
-        self._w = None
 
-    input_buffer = CausalConv3d.input_buffer
-    run = CausalConv3d.run
+    def input_buffer(self, x_shape, dtype, device):
+        return conv_buffer(self, x_shape, dtype, device)
+
+    def run(self, buf, resid=None):
+        return run_conv(self, buf, resid)
 
 
 class ResnetBlock3D(nn.Module):
@@ -107,12 +85,12 @@ class ResnetBlock3D(nn.Module):
 
     def forward(self, x):
         buf = self.conv1.input_buffer(x.shape, x.dtype, x.device)
-        _gn(self.norm1, x, buf, t_off=2)
+        group_norm(self.norm1, x, buf, t_off=2, act=True)
         h = self.conv1.run(buf)
         buf = self.conv2.input_buffer(h.shape, h.dtype, h.device)
-        _gn(self.norm2, h, buf, t_off=2)
+        group_norm(self.norm2, h, buf, t_off=2, act=True)
         if self.in_channels != self.out_channels:
-            x = kernels.gemm_bias_act(x, self.nin_shortcut._w, self.nin_shortcut.bias)
+            x = kernels.gemm_bias_act(x, self.nin_shortcut.conv._w, self.nin_shortcut.conv._b)
         return self.conv2.run(buf, resid=x)
 
 
@@ -134,19 +112,14 @@ class AttnBlock3DFix(nn.Module):
         self.proj_out = CausalConv3d(in_channels, in_channels, kernel_size=1, stride=1)
         self._w_qkv = self._b_qkv = None
 
+    def pack(self):
+        qkv = [self.q.conv, self.k.conv, self.v.conv]
+        self._w_qkv = torch.cat([c.weight for c in qkv]).flatten(1).detach().contiguous()
+        self._b_qkv = torch.cat([c.bias for c in qkv]).detach().contiguous()
+
     def forward(self, x):
-        B, T, H, W, C = x.shape
-        qkv = kernels.gemm_bias_act(_gn(self.norm, x, act=False), self._w_qkv, self._b_qkv)
-        q, k, vt = kernels.vae_attn_split(qkv, C, self.mixed)
-        P, Pp = H * W, k.shape[1]
-        o = torch.empty(B * T, P, C, dtype=x.dtype, device=x.device)
-        s = torch.empty(P, Pp, dtype=x.dtype, device=x.device)  # one frame's scores at a time
-        for f in range(B * T):
-            kernels.gemm_bias_act(q[f], k[f], out=s)
-            kernels.vae_attn_softmax_(s, P, int(C) ** (-0.5))
-            kernels.gemm_bias_act(s, vt[f], out=o[f])
-        o = kernels.vae_attn_merge(o, B, T, H, W) if self.mixed else o.view(B, T, H, W, C)
-        return kernels.gemm_bias_residual(o, self.proj_out._w, self.proj_out.bias, x, out=torch.empty_like(x))
+        out = self.proj_out.conv
+        return attention(x, self.norm, self._w_qkv, self._b_qkv, out._w, out._b, self.mixed)
 
 
 class AttnBlock3D(AttnBlock3DFix):
@@ -200,6 +173,10 @@ class TimeUpsampleRes2x(nn.Module):
         self.conv = CausalConv3d(in_channels, out_channels, kernel_size, padding=1)
         self.mix_factor = nn.Parameter(torch.Tensor([mix_factor]))
         self._alpha = None
+
+    def pack(self):
+        alpha = torch.sigmoid(self.mix_factor.detach())
+        self._alpha = (float(alpha), float(1 - alpha))
 
     def forward(self, x):
         B, T, H, W, C = x.shape
@@ -264,13 +241,13 @@ class Decoder(nn.Module):
             if hasattr(up, "time_upsample"):
                 h = up.time_upsample(h)
         buf = self.conv_out.input_buffer(h.shape, h.dtype, h.device)
-        _gn(self.norm_out, h, buf, t_off=self.conv_out.time_kernel_size - 1)
+        group_norm(self.norm_out, h, buf, t_off=self.conv_out.time_kernel_size - 1, act=True)
         return self.conv_out.run(buf)
 
 
-class _CausalVAEDecoderModel(nn.Module):
-    """The decoder half of CausalVAEModel, shared by both versions.  ``load_state_dict`` takes the reference's full state
-    dict: it drops ``encoder.*``, ``quant_conv.*`` and ``loss.*`` and is strict about every other key."""
+class _CausalVAEDecoderModel(DecoderOnlyVAE):
+    """The decoder half of CausalVAEModel, shared by both versions.  ``load_state_dict`` drops the ``encoder.*``,
+    ``quant_conv.*`` and ``loss.*`` entries of the reference's full state dict."""
 
     _DROPPED_PREFIXES = ("encoder.", "quant_conv.", "loss.")
     _ACCEPTED = {}  # decoder slot -> accepted module names
@@ -294,12 +271,10 @@ class _CausalVAEDecoderModel(nn.Module):
         if len(cfg["decoder_resnet_blocks"]) != len(mult) or len(cfg["decoder_spatial_upsample"]) != len(mult) or \
                 len(cfg["decoder_temporal_upsample"]) != len(mult):
             raise ValueError("decoder_resnet_blocks / _spatial_upsample / _temporal_upsample need one entry per hidden_size_mult")
-        for m in mult:
-            if cfg["hidden_size"] * m not in _GN_CHANNELS:
-                raise ValueError(f"hidden_size={cfg['hidden_size']} x hidden_size_mult {mult}: each width must be one of {_GN_CHANNELS}")
+        check_widths([cfg["hidden_size"] * m for m in mult], f"hidden_size={cfg['hidden_size']} x hidden_size_mult {mult}")
         for k in ("z_channels", "embed_dim"):
-            if not 0 < cfg[k] <= _LATENT_PAD:
-                raise ValueError(f"{k}={cfg[k]}: the decoder pads the latent to {_LATENT_PAD} channels (need 1 .. 16)")
+            if not 0 < cfg[k] <= LATENT_PAD:
+                raise ValueError(f"{k}={cfg[k]}: the decoder pads the latent to {LATENT_PAD} channels (need 1 .. 16)")
         self.use_quant_layer = use_quant_layer
         self.decoder = Decoder(cfg["z_channels"], cfg["hidden_size"], mult, cfg["decoder_conv_in"], cfg["decoder_conv_out"],
                                cfg["decoder_attention"], cfg["decoder_resnet_blocks"], cfg["decoder_spatial_upsample"],
@@ -307,14 +282,8 @@ class _CausalVAEDecoderModel(nn.Module):
         if use_quant_layer:
             self.post_quant_conv = CausalConv3d(cfg["embed_dim"], cfg["z_channels"], 1)
         self.use_tiling = False
-        self._pack_key = None
 
     # ---- loading ----
-    @classmethod
-    def from_config(cls, cfg: dict):
-        keys = set(inspect.signature(cls.__init__).parameters) - {"self"}
-        return cls(**{k: v for k, v in cfg.items() if k in keys})
-
     @classmethod
     def from_pretrained(cls, path: str, subfolder: Optional[str] = None):
         """A LOCAL directory (``path`` / ``subfolder``): its last ``*.ckpt`` with ``config.json`` next to it (the
@@ -335,10 +304,6 @@ class _CausalVAEDecoderModel(nn.Module):
         raise FileNotFoundError(f"{cls.__name__}.from_pretrained: no *.ckpt in {os.path.join(path, subfolder or '')} "
                                 "(local directories only)")
 
-    def load_state_dict(self, state_dict, strict: bool = True):
-        kept = {k: v for k, v in state_dict.items() if not k.startswith(self._DROPPED_PREFIXES)}
-        return super().load_state_dict(kept, strict=strict)
-
     @property
     def dtype(self):
         return self.decoder.norm_out.weight.dtype
@@ -349,40 +314,15 @@ class _CausalVAEDecoderModel(nn.Module):
     def disable_tiling(self):
         self.enable_tiling(False)
 
-    def encode(self, x):
-        raise NotImplementedError(f"{type(self).__name__}.encode: the VAE encoder is out of scope (decoder only)")
-
     # ---- kernel weights ----
-    def _pack_weights(self):
-        """Packs the weights for the kernels once per set of parameter tensors (after loading, .to(), ...)."""
-        key = tuple((p.data_ptr(), p._version, p.dtype, p.device) for p in self.parameters())
-        if key == self._pack_key:
-            return
-        for m in self.modules():
-            if isinstance(m, (CausalConv3d, Conv2d)):
-                w = m.weight.detach()
-                m._w = kernels.pack_conv_weight(w) if w.shape[-1] == 3 else w.flatten(1).contiguous()
-            elif isinstance(m, AttnBlock3DFix):
-                m._w_qkv = torch.cat([m.q.weight, m.k.weight, m.v.weight]).flatten(1).detach().contiguous()
-                m._b_qkv = torch.cat([m.q.bias, m.k.bias, m.v.bias]).detach().contiguous()
-            elif isinstance(m, TimeUpsampleRes2x):
-                alpha = torch.sigmoid(m.mix_factor.detach())
-                m._alpha = (float(alpha), float(1 - alpha))
+    def pack(self):
         if self.use_quant_layer:
-            pq = self.post_quant_conv
-            w = torch.zeros(_LATENT_PAD, _LATENT_PAD, dtype=pq.weight.dtype, device=pq.weight.device)
-            w[:pq.chan_out, :pq.chan_in] = pq.weight.detach().flatten(1)
-            b = torch.zeros(_LATENT_PAD, dtype=pq.weight.dtype, device=pq.weight.device)
-            b[:pq.chan_out] = pq.bias.detach()
-            self._pq = (w, b)
-        self._pack_key = key
+            self._pq = pad_1x1(self.post_quant_conv.conv.weight, self.post_quant_conv.conv.bias)
 
     # ---- decoding ----
     def _decode_tile(self, z):
         """post_quant_conv + decoder of z [B, Cz, T, h, w] -> [B, 3, T', 8h, 8w] (reference decode without tiling)."""
-        B, Cz, T, h, w = z.shape
-        zp = torch.zeros(B, T, h, w, _LATENT_PAD, dtype=z.dtype, device=z.device)
-        zp[..., :Cz] = z.permute(0, 2, 3, 4, 1)
+        zp = pad_latent(z.permute(0, 2, 3, 4, 1))
         if self.use_quant_layer:
             zp = kernels.gemm_bias_act(zp, *self._pq)
         return self.decoder(zp).permute(0, 4, 1, 2, 3)
@@ -390,26 +330,11 @@ class _CausalVAEDecoderModel(nn.Module):
     @torch.no_grad()
     def decode(self, z):
         """z [B, embed_dim, T, h, w] -> [B, 3, T', 8h, 8w] (the reference's CausalVAEModel.decode)."""
-        kernels.require_cuda(z, f"{type(self).__name__}.decode")
-        z = z.to(self.dtype)
-        kernels.require_cuda(z, f"{type(self).__name__}.decode", half_only=True)
-        self._pack_weights()
+        z = self._decode_input(z)
         if self.use_tiling and (z.shape[-1] > self.tile_latent_min_size or z.shape[-2] > self.tile_latent_min_size
                                 or z.shape[-3] > self.tile_latent_min_size_t):
             return self.tiled_decode(z)
         return self._decode_tile(z)
-
-    def blend_v(self, a, b, blend_extent: int):
-        blend_extent = min(a.shape[3], b.shape[3], blend_extent)
-        for y in range(blend_extent):
-            b[:, :, :, y, :] = a[:, :, :, -blend_extent + y, :] * (1 - y / blend_extent) + b[:, :, :, y, :] * (y / blend_extent)
-        return b
-
-    def blend_h(self, a, b, blend_extent: int):
-        blend_extent = min(a.shape[4], b.shape[4], blend_extent)
-        for x in range(blend_extent):
-            b[:, :, :, :, x] = a[:, :, :, :, -blend_extent + x] * (1 - x / blend_extent) + b[:, :, :, :, x] * (x / blend_extent)
-        return b
 
     def tiled_decode(self, x):
         t = x.shape[2]
@@ -429,27 +354,8 @@ class _CausalVAEDecoderModel(nn.Module):
         return torch.cat(dec_, dim=2)
 
     def tiled_decode2d(self, z):
-        overlap_size = int(self.tile_latent_min_size * (1 - self.tile_overlap_factor))
-        blend_extent = int(self.tile_sample_min_size * self.tile_overlap_factor)
-        row_limit = self.tile_sample_min_size - blend_extent
-        rows = []
-        for i in range(0, z.shape[3], overlap_size):
-            row = []
-            for j in range(0, z.shape[4], overlap_size):
-                tile = z[:, :, :, i:i + self.tile_latent_min_size, j:j + self.tile_latent_min_size]
-                row.append(self._decode_tile(tile))
-            rows.append(row)
-        result_rows = []
-        for i, row in enumerate(rows):
-            result_row = []
-            for j, tile in enumerate(row):
-                if i > 0:
-                    tile = self.blend_v(rows[i - 1][j], tile, blend_extent)
-                if j > 0:
-                    tile = self.blend_h(row[j - 1], tile, blend_extent)
-                result_row.append(tile[:, :, :, :row_limit, :row_limit])
-            result_rows.append(torch.cat(result_row, dim=4))
-        return torch.cat(result_rows, dim=3)
+        return tiled_decode_2d(z, lambda tile: self._decode_tile(tile), (self.tile_latent_min_size,) * 2,
+                               (self.tile_sample_min_size,) * 2, (self.tile_overlap_factor,) * 2)
 
 
 _V120_ACCEPTED = {"conv_in": _CONVS, "conv_out": _CONVS, "attention": ("AttnBlock3DFix",), "resnet_blocks": _RESNETS,
@@ -535,12 +441,7 @@ class CausalVAEModelV110(_CausalVAEDecoderModel):
     @classmethod
     def _from_diffusers_weights(cls, path, subfolder):
         """Without a *.ckpt the reference falls back to ModelMixin.from_pretrained: config.json + diffusers weights."""
-        from ...utils.checkpoint import load_local_checkpoint
-
-        cfg, sd = load_local_checkpoint(path, subfolder or "")
-        vae = cls.from_config(cfg)
-        vae.load_state_dict(sd)
-        return vae
+        return cls._from_local_diffusers(path, subfolder or "")
 
 
 def decoder_class(version: str):
