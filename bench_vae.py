@@ -2,7 +2,7 @@
 of the same modules (the stand-ins of tests/kernels_emul_vae.py, which compute what the reference's eager decoders
 compute), in alternating rounds after a warm-up round.
 
-    python bench_vae.py [--rounds 3] [cogvideox|osp|opensora ...]    (all three by default)
+    python bench_vae.py [--rounds 3] [cogvideox|osp|opensora|latte|vchitect ...]    (all by default)
 
 Workloads, random weights:
   - cogvideox: latents [1, 16, 13, 60, 90] (CogVideoX-2b, 49 frames at 480 x 720), fp16, released widths; decoded tiled
@@ -16,8 +16,15 @@ Workloads, random weights:
     the launches of one native decode:
       720p 9:16, 68 frames: latents [1, 4, 20, 90, 160];
       240p 9:16, 51 frames: latents [1, 4, 15, 30, 53].
-Prints the card and its power limit, then one JSON line per model.  For Open-Sora-Plan and OpenSora the decoded frames of
-the two chains are compared.
+  - latte: fp16, released widths, latents [1, 4, 16, 64, 64] (16 frames at 512 x 512) as LattePipeline decodes them:
+    the SVD temporal decoder on chunks of 14 + 2 frames, and the image VAE (enable_vae_temporal_decoder=False); then the
+    rates of the time-axis convolution at the temporal decoder's top level (128 channels, 512 x 512, 14 frames): plain,
+    with the residual + AlphaBlender epilogue, and the same result unfused (residual epilogue, then a vae_mix pass).
+  - vchitect: bf16, released widths, 16 latent channels, latents [1, 40, 16, 36, 60] (40 frames at 288 x 480), decoded as
+    VchitectXLPipeline does (several frames per pass).
+For OpenSora, Latte and Vchitect the FLOPs of the convolutions and GEMMs are counted from the shapes of the launches of
+one native decode.  Prints the card and its power limit, then one JSON line per model.  For Open-Sora-Plan, OpenSora,
+Latte and Vchitect the decoded frames of the two chains are compared.
 """
 import argparse
 import contextlib
@@ -28,10 +35,12 @@ import time
 import torch
 
 from oracle import gen_golden_cogvideox_vae as GC, gen_golden_opensora_vae as GS, gen_golden_osp_vae as GP
-from tests import kernels_emul_vae as EV
+from oracle import gen_golden_latte_vae as GL
+from tests import kernels_emul_vae_time as EV
 from videosys_b200 import kernels
-from videosys_b200.models.autoencoders import (AutoencoderKLCogVideoX, CausalVAEModelV110, CausalVAEModelV120,
-                                               VideoAutoencoderPipeline)
+from videosys_b200.models.autoencoders import (AutoencoderKL, AutoencoderKLCogVideoX, AutoencoderKLTemporalDecoder,
+                                               CausalVAEModelV110, CausalVAEModelV120, VideoAutoencoderPipeline)
+from videosys_b200.pipelines._common import decode_image_frames
 
 
 # ---- the shared harness ----
@@ -217,7 +226,81 @@ def opensora(rounds):
     return result
 
 
-MODELS = {"cogvideox": cogvideox, "osp": osp, "opensora": opensora}
+# ---- Latte and Vchitect-2.0 ----
+def _flops(decode):
+    """FLOPs of the convolutions and GEMMs of one native decode, from the launches' shapes."""
+    kernels.PROFILE, kernels.PROFILE_KINDS = [], {"vae_conv3d", "vae_conv_time", "gemm"}
+    try:
+        decode()
+        torch.cuda.synchronize()
+        return sum(w for _, _, _, w in kernels.PROFILE)
+    finally:
+        kernels.PROFILE, kernels.PROFILE_KINDS = None, None
+
+
+def _run(tag, decode, rounds):
+    flop = _flops(decode)
+    tn, te, ours, ref = _rounds(decode, rounds)
+    res = {"frames": list(ours.shape), **_times(tn, te), "tflop": round(flop / 1e12, 2),
+           "native_tflops": round(flop / 1e12 / (min(tn) / 1e3), 1), "eager_tflops": round(flop / 1e12 / (min(te) / 1e3), 1),
+           **_diff(ours, ref)}
+    print(f"[{tag}] {tuple(ours.shape)}: {flop / 1e12:.2f} TFLOP; native {min(tn):.1f} ms ({res['native_tflops']} TFLOP/s), "
+          f"eager {min(te):.1f} ms ({res['eager_tflops']} TFLOP/s); |native - eager| max {res['max_abs_diff']:.4f}, "
+          f"mean {res['mean_abs_diff']:.2e} (on the [-1, 1] scale)")
+    return res
+
+
+def conv_time_rates(dt):
+    """ms and TFLOP/s of vae_conv_time at the temporal decoder's top level, with and without the mix epilogue."""
+    g = torch.Generator(device="cuda").manual_seed(0)
+    T, H, W, C = 14, 512, 512, 128
+    x = torch.randn(1, T + 2, H, W, C, device="cuda", generator=g).to(dt)
+    xs = torch.randn(1, T, H, W, C, device="cuda", generator=g).to(dt)
+    wp = kernels.pack_conv_weight((0.05 * torch.randn(C, C, 3, 1, 1, device="cuda", generator=g)).to(dt))
+    b = torch.zeros(C, device="cuda", dtype=dt)
+    flop = 2 * T * H * W * C * C * 3
+    res = {}
+    for name, kw in (("conv_time_128_512x512_t14", {}), ("conv_time_mix_128_512x512_t14", dict(resid=xs, mix=(0.25, 0.75)))):
+        ms = _events(lambda: kernels.vae_conv_time(x, wp, b, C, 3, **kw), 10)
+        res[name] = {"ms": round(ms, 3), "tflops": round(flop / ms / 1e9, 1)}
+    # the same result unfused: the residual in the conv epilogue, then the AlphaBlender as a separate vae_mix pass
+    ms = _events(lambda: kernels.vae_mix(xs, kernels.vae_conv_time(x, wp, b, C, 3, resid=xs), 0.25, 0.75), 10)
+    res["conv_time_resid_then_vae_mix_128_512x512_t14"] = {"ms": round(ms, 3), "tflops": round(flop / ms / 1e9, 1)}
+    return res
+
+
+def latte(rounds):
+    dt = torch.float16
+    z = (torch.randn(1, 4, 16, 64, 64, generator=torch.Generator().manual_seed(0)) / 0.18215).to(dt).cuda()
+    frames = z.permute(0, 2, 1, 3, 4).reshape(16, 4, 64, 64)  # the pipeline's (b f) c h w, already scaled
+    result = {"workload": "latte_vae_decode_1x4x16x64x64_fp16"}
+    for key, cls in (("temporal_decoder", AutoencoderKLTemporalDecoder), ("sd_vae", AutoencoderKL)):
+        vae = cls()
+        vae.load_state_dict(GS.weights(vae.state_dict(), "released"))
+        vae = vae.to(dt).cuda().eval()
+        if cls is AutoencoderKLTemporalDecoder:  # LattePipeline.decode_video: chunks of 14 frames
+            decode = lambda: torch.cat([vae.decode(frames[i:i + 14], num_frames=len(frames[i:i + 14])).sample  # noqa: E731
+                                        for i in range(0, 16, 14)])
+        else:
+            decode = lambda: decode_image_frames(vae, frames)  # noqa: E731
+        result[key] = _run(f"latte {key}", decode, rounds)
+        del vae
+        torch.cuda.empty_cache()
+    result["kernels"] = conv_time_rates(dt)
+    return result
+
+
+def vchitect(rounds):
+    dt = torch.bfloat16
+    vae = AutoencoderKL(latent_channels=16, use_post_quant_conv=False)
+    vae.load_state_dict(GS.weights(vae.state_dict(), "released"))
+    vae = vae.to(dt).cuda().eval()
+    z = torch.randn(1, 40, 16, 36, 60, generator=torch.Generator().manual_seed(0)).to(dt).cuda()
+    z = (z / GL.VCH_SCALE) + GL.VCH_SHIFT
+    return {"workload": "vchitect_vae_decode_1x40x16x36x60_bf16", **_run("vchitect", lambda: decode_image_frames(vae, z[0]), rounds)}
+
+
+MODELS = {"cogvideox": cogvideox, "osp": osp, "opensora": opensora, "latte": latte, "vchitect": vchitect}
 
 
 def main():

@@ -326,6 +326,26 @@ int vsb_vae_attn_merge(const vsb_bf16* o, vsb_bf16* out, int B, int T, int P, in
 int vsb_vae_depth_to_time(const vsb_bf16* x, vsb_bf16* out, int B, int T, int H, int W, int C, int t_off, int T_out,
                           void* stream);
 
+/* ---- SVD temporal decoder (Latte's vae_temporal_decoder, models/autoencoders/autoencoder_kl_temporal_decoder.py) -----
+ * The per-frame ResnetBlock2D halves, the mid-block attention and the up-samplers run on the entries above; the
+ * TemporalResnetBlock halves and time_conv_out run on:
+ * vsb_vae_conv_time: a (kt, 1, 1) convolution of x [B, kt-1+T, H, W, Cin] (channels-last; a zero-padded input with
+ *   padding (1, 0, 0) is frames 1 .. T of a buffer whose frames 0 and T+1 are zero) on the implicit GEMM of
+ *   vsb_vae_conv3d with one spatial tap: K = kt * Cin, the A box only moves in time.  w_packed [Cout, kt, Cin] (tap-major,
+ *   kernels.pack_conv_weight of a [Cout, Cin, kt, 1, 1] weight).  v = bf16(bf16(conv) + bias) with round_conv (else
+ *   bf16(conv + bias)); mix = 0: out = v [+ resid, rounded]; mix = 1 (TemporalResnetBlock.conv2 + AlphaBlender):
+ *   xt = bf16(resid + v), out = bf16(bf16(mix_a * resid) + bf16(mix_b * xt)), resid [B, T, H, W, Cout] being the spatial
+ *   block's output and mix_a / mix_b 16-bit values (1 - sigmoid(mix_factor) and 1 - that, rounded on the host).
+ *   Cin and Cout multiples of 64.
+ * vsb_vae_time_conv_rgb: time_conv_out, Conv3d 3 -> 3 with kernel (3, 1, 1), padding (1, 0, 0) and bias, of x [B, T, H,
+ *   W, 3] -> out [B, T, H, W, 3]; w is the Conv3d weight [3, 3, 3, 1, 1] as stored.  Each output: the 9 products summed
+ *   in fp32, rounded, + bias, rounded (as vsb_vae_conv3d with round_conv). */
+int vsb_vae_conv_time(const vsb_bf16* x, const vsb_bf16* w_packed, const vsb_bf16* bias, const vsb_bf16* resid, vsb_bf16* out,
+                      int B, int T, int H, int W, int Cin, int Cout, int kt, int mix, float mix_a, float mix_b, int round_conv,
+                      void* stream);
+int vsb_vae_time_conv_rgb(const vsb_bf16* x, const vsb_bf16* w, const vsb_bf16* bias, vsb_bf16* out, int B, int T, int H,
+                          int W, void* stream);
+
 /* ---- IEEE fp16 twins ----------------------------------------------------------------------------------------------
  * The reference runs CogVideoX-2b and Latte in torch.float16 (pipelines/cogvideox/pipeline_cogvideox.py:138-139,
  * pipelines/latte/pipeline_latte.py:201).  Every kernel entry above that touches activations exists a second time with
@@ -399,6 +419,11 @@ int vsb_vae_attn_softmax_f16(vsb_f16* S, int rows, int P, int Pp, float scale, v
 int vsb_vae_attn_merge_f16(const vsb_f16* o, vsb_f16* out, int B, int T, int P, int C, void* stream);
 int vsb_vae_depth_to_time_f16(const vsb_f16* x, vsb_f16* out, int B, int T, int H, int W, int C, int t_off, int T_out,
                               void* stream);
+int vsb_vae_conv_time_f16(const vsb_f16* x, const vsb_f16* w_packed, const vsb_f16* bias, const vsb_f16* resid, vsb_f16* out,
+                          int B, int T, int H, int W, int Cin, int Cout, int kt, int mix, float mix_a, float mix_b,
+                          int round_conv, void* stream);
+int vsb_vae_time_conv_rgb_f16(const vsb_f16* x, const vsb_f16* w, const vsb_f16* bias, vsb_f16* out, int B, int T, int H,
+                              int W, void* stream);
 
 #ifdef __cplusplus
 }

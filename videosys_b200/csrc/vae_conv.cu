@@ -14,6 +14,9 @@
 //   epilogue        + bias (rounded the way torch's convolution rounds, see round_conv), optional + residual, masked
 //                   stores of the valid pixels and the Cout real channels (Cout = 3 for conv_out, 4 for the OpenSora
 //                   temporal decoder's).
+// TAPS is the number of spatial taps per frame: 9 for the (kt, 3, 3) convolutions, 1 for the (kt, 1, 1) time-axis
+// convolution of the SVD temporal decoder (vsb_vae_conv_time), where only the A box's frame coordinate moves per tap.
+// MIX adds that decoder's residual and AlphaBlender to the epilogue (see vsb_vae_conv_time).
 #include "vsb_common.cuh"
 #include "vsb_host.h"
 #include "wgmma.cuh"
@@ -48,11 +51,13 @@ struct ConvArgs {
   const bf16* resid;  // [B, T, H, W, Cout] or null
   bf16* out;          // [B, T, H, W, Cout]
   int T, H, W, Cout, kt, cin_slices, tiles_h, tiles_w, tiles_n, round_conv;
+  float mix_a, mix_b;  // MIX only: the AlphaBlender's weights of resid and of resid + conv
 };
 
-template <int BN>
+template <int BN, int TAPS = 9, bool MIX = false>
 __global__ void __launch_bounds__(kConvThreads, 1)
 vae_conv_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_w, const ConvArgs a) {
+  static_assert(TAPS == 9 || TAPS == 1, "3x3 or 1x1 spatial taps");
   using Cfg = ConvCfg<BN>;
   extern __shared__ unsigned char smem_dyn[];
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~uintptr_t(1023));
@@ -68,7 +73,7 @@ vae_conv_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant_
   const int h0 = (r % a.tiles_h) * kConvBH;
   r /= a.tiles_h;
   const int t = r % a.T, b = r / a.T;
-  const int taps = a.kt * 9;
+  const int taps = a.kt * TAPS;
   const int num_kb = taps * a.cin_slices;
   const int wg = threadIdx.x >> 7;
 
@@ -87,7 +92,7 @@ vae_conv_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant_
     if (threadIdx.x == 0) {
       int kb = 0;
       for (int tap = 0; tap < taps; ++tap) {
-        const int dz = tap / 9, dy = (tap / 3) % 3 - 1, dx = tap % 3 - 1;
+        const int dz = tap / TAPS, dy = TAPS == 9 ? (tap / 3) % 3 - 1 : 0, dx = TAPS == 9 ? tap % 3 - 1 : 0;
         for (int cs = 0; cs < a.cin_slices; ++cs, ++kb) {
           const int s = kb % kConvStages;
           mbar_wait_quiet(&empty[s], ((kb / kConvStages) & 1) ^ 1);
@@ -148,7 +153,12 @@ vae_conv_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant_
       x0 = rbf(x0 + b0);
       x1 = rbf(x1 + b1);
       const size_t off = (size_t)pix[h] * a.Cout + col;
-      if (a.resid != nullptr) {  // ResNet sum conv2(...) + inputs (:298), its own eager rounding
+      if constexpr (MIX) {  // xt = xs + v, then a * xs + b * xt, each eager op rounded (Cout % 64 == 0: both columns)
+        const float2 sp = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(a.resid + off));
+        const float s0 = sp.x, s1 = sp.y;
+        x0 = rbf(rbf(a.mix_a * s0) + rbf(a.mix_b * rbf(s0 + x0)));
+        x1 = rbf(rbf(a.mix_a * s1) + rbf(a.mix_b * rbf(s1 + x1)));
+      } else if (a.resid != nullptr) {  // ResNet sum conv2(...) + inputs (:298), its own eager rounding
         x0 += e_to_float(a.resid[off]);
         if (two) x1 += e_to_float(a.resid[off + 1]);
       }
@@ -162,18 +172,52 @@ vae_conv_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant_
   }
 }
 
-template <int BN>
+template <int BN, int TAPS = 9, bool MIX = false>
 int launch_conv(const CUtensorMap& tx, const CUtensorMap& tw, const ConvArgs& a, int B, cudaStream_t st) {
+  const char* what = TAPS == 9 ? "vae_conv3d" : "vae_conv_time";
   static bool attr = false;
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(vae_conv_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, ConvCfg<BN>::kSmemBytes);
-    if (e != cudaSuccess) return fail(VSB_ERR_CUDA, "vae_conv3d: smem attr: %s", cudaGetErrorString(e));
+    cudaError_t e = cudaFuncSetAttribute(vae_conv_kernel<BN, TAPS, MIX>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         ConvCfg<BN>::kSmemBytes);
+    if (e != cudaSuccess) return fail(VSB_ERR_CUDA, "%s: smem attr: %s", what, cudaGetErrorString(e));
     attr = true;
   }
   const long long tiles = (long long)B * a.T * a.tiles_h * a.tiles_w * a.tiles_n;
-  if (tiles >= (1ll << 31)) return fail(VSB_ERR_UNSUPPORTED, "vae_conv3d: too many tiles");
-  vae_conv_kernel<BN><<<(unsigned)tiles, kConvThreads, ConvCfg<BN>::kSmemBytes, st>>>(tx, tw, a);
-  return check_launch("vae_conv3d");
+  if (tiles >= (1ll << 31)) return fail(VSB_ERR_UNSUPPORTED, "%s: too many tiles", what);
+  vae_conv_kernel<BN, TAPS, MIX><<<(unsigned)tiles, kConvThreads, ConvCfg<BN>::kSmemBytes, st>>>(tx, tw, a);
+  return check_launch(what);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// time_conv_out of the SVD temporal decoder: Conv3d 3 -> 3, kernel (3, 1, 1), zero frames at both ends, one thread per
+// pixel.  Each output is the 9 products summed in fp32 (frame-major, then input channel), rounded, + bias, rounded.
+// ---------------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) time_conv_rgb_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w,
+                                                            const bf16* __restrict__ bias, bf16* __restrict__ out, int B,
+                                                            int T, long long P) {
+  __shared__ float ws[27], bs[3];
+  if (threadIdx.x < 27) ws[threadIdx.x] = e_to_float(w[threadIdx.x]);  // [Cout, Cin, kt]
+  if (threadIdx.x < 3) bs[threadIdx.x] = e_to_float(bias[threadIdx.x]);
+  __syncthreads();
+  const long long total = (long long)B * T * P;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int t = (int)((i / P) % T);
+    float acc[3] = {0.f, 0.f, 0.f};
+#pragma unroll
+    for (int dz = 0; dz < 3; ++dz) {
+      const int ts = t + dz - 1;
+      if (ts < 0 || ts >= T) continue;
+      const bf16* src = x + (i + (long long)(dz - 1) * P) * 3;
+#pragma unroll
+      for (int ci = 0; ci < 3; ++ci) {
+        const float v = e_to_float(src[ci]);
+#pragma unroll
+        for (int co = 0; co < 3; ++co) acc[co] = fmaf(ws[(co * 3 + ci) * 3 + dz], v, acc[co]);
+      }
+    }
+#pragma unroll
+    for (int co = 0; co < 3; ++co) out[i * 3 + co] = float_to_e(rbf(acc[co]) + bs[co]);
+  }
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -380,6 +424,27 @@ int grid_for(long long work) {
 
 using namespace vsb;
 
+namespace vsb {
+namespace {
+// The two TMA operands of vae_conv_kernel: x [B, Tin, H, W, Cin] as 64-channel x 16 x 8 x 1 x 1 boxes and the packed
+// weight [Cout_pad, K] as 64 x BN boxes, both 128B-swizzled.
+int conv_tmaps(CUtensorMap* tx, CUtensorMap* tw, const void* x, const void* w_packed, int B, int Tin, int H, int W, int Cin,
+               unsigned long long K, int cout_pad, int BN) {
+  unsigned long long dx[5] = {(unsigned long long)Cin, (unsigned long long)W, (unsigned long long)H, (unsigned long long)Tin,
+                              (unsigned long long)B};
+  unsigned long long sx[4] = {(unsigned long long)Cin * 2, (unsigned long long)W * Cin * 2,
+                              (unsigned long long)H * W * Cin * 2, (unsigned long long)Tin * H * W * Cin * 2};
+  unsigned bx[5] = {kConvBK, kConvBW, kConvBH, 1, 1};
+  int rc = make_tmap_bf16(tx, x, 5, dx, sx, bx, CU_TENSOR_MAP_SWIZZLE_128B);
+  if (rc) return rc;
+  unsigned long long dw[2] = {K, (unsigned long long)cout_pad};
+  unsigned long long sw[1] = {K * 2};
+  unsigned bw[2] = {kConvBK, (unsigned)BN};
+  return make_tmap_bf16(tw, w_packed, 2, dw, sw, bw, CU_TENSOR_MAP_SWIZZLE_128B);
+}
+}  // namespace
+}  // namespace vsb
+
 extern "C" int VSB_API(vsb_vae_conv3d)(const vsb_bf16* x, const vsb_bf16* w_packed, const vsb_bf16* bias, const vsb_bf16* resid,
                                        vsb_bf16* out, int B, int T, int H, int W, int Cin, int Cout, int kt, int round_conv,
                                        void* stream) {
@@ -393,25 +458,43 @@ extern "C" int VSB_API(vsb_vae_conv3d)(const vsb_bf16* x, const vsb_bf16* w_pack
     return fail(VSB_ERR_UNSUPPORTED, "vae_conv3d: misaligned pointer");
   const int BN = Cout % 128 == 0 ? 128 : 64;
   const int cin_pad = (Cin + 63) / 64 * 64, cout_pad = (Cout + BN - 1) / BN * BN;
-  const int Tin = T + kt - 1;
   CUtensorMap tx, tw;
-  unsigned long long dx[5] = {(unsigned long long)Cin, (unsigned long long)W, (unsigned long long)H, (unsigned long long)Tin,
-                              (unsigned long long)B};
-  unsigned long long sx[4] = {(unsigned long long)Cin * 2, (unsigned long long)W * Cin * 2,
-                              (unsigned long long)H * W * Cin * 2, (unsigned long long)Tin * H * W * Cin * 2};
-  unsigned bx[5] = {kConvBK, kConvBW, kConvBH, 1, 1};
-  int rc = make_tmap_bf16(&tx, x, 5, dx, sx, bx, CU_TENSOR_MAP_SWIZZLE_128B);
-  if (rc) return rc;
-  const unsigned long long K = (unsigned long long)kt * 9 * cin_pad;
-  unsigned long long dw[2] = {K, (unsigned long long)cout_pad};
-  unsigned long long sw[1] = {K * 2};
-  unsigned bw[2] = {kConvBK, (unsigned)BN};
-  rc = make_tmap_bf16(&tw, w_packed, 2, dw, sw, bw, CU_TENSOR_MAP_SWIZZLE_128B);
+  int rc = conv_tmaps(&tx, &tw, x, w_packed, B, T + kt - 1, H, W, Cin, (unsigned long long)kt * 9 * cin_pad, cout_pad, BN);
   if (rc) return rc;
   ConvArgs a{(const bf16*)bias, (const bf16*)resid, (bf16*)out, T, H, W, Cout, kt, cin_pad / 64,
-             (H + kConvBH - 1) / kConvBH, (W + kConvBW - 1) / kConvBW, cout_pad / BN, round_conv ? 1 : 0};
+             (H + kConvBH - 1) / kConvBH, (W + kConvBW - 1) / kConvBW, cout_pad / BN, round_conv ? 1 : 0, 0.f, 0.f};
   if (BN == 128) return launch_conv<128>(tx, tw, a, B, (cudaStream_t)stream);
   return launch_conv<64>(tx, tw, a, B, (cudaStream_t)stream);
+}
+
+extern "C" int VSB_API(vsb_vae_conv_time)(const vsb_bf16* x, const vsb_bf16* w_packed, const vsb_bf16* bias,
+                                          const vsb_bf16* resid, vsb_bf16* out, int B, int T, int H, int W, int Cin, int Cout,
+                                          int kt, int mix, float mix_a, float mix_b, int round_conv, void* stream) {
+  if (!x || !w_packed || !bias || !out || B <= 0 || T <= 0 || H <= 0 || W <= 0 || Cin <= 0 || Cout <= 0 || kt <= 0 ||
+      (mix && !resid))
+    return fail(VSB_ERR_INVALID, "vae_conv_time: bad args");
+  if (Cin % 64 || Cout % 64)
+    return fail(VSB_ERR_UNSUPPORTED, "vae_conv_time: Cin=%d Cout=%d (need multiples of 64)", Cin, Cout);
+  if (!aligned16(x) || !aligned16(w_packed) || (resid && ((uintptr_t)resid & 3)) || ((uintptr_t)out & 3))
+    return fail(VSB_ERR_UNSUPPORTED, "vae_conv_time: misaligned pointer");
+  const int BN = Cout % 128 == 0 ? 128 : 64;
+  CUtensorMap tx, tw;
+  int rc = conv_tmaps(&tx, &tw, x, w_packed, B, T + kt - 1, H, W, Cin, (unsigned long long)kt * Cin, Cout, BN);
+  if (rc) return rc;
+  ConvArgs a{(const bf16*)bias, (const bf16*)resid, (bf16*)out, T, H, W, Cout, kt, Cin / 64,
+             (H + kConvBH - 1) / kConvBH, (W + kConvBW - 1) / kConvBW, Cout / BN, round_conv ? 1 : 0, mix_a, mix_b};
+  cudaStream_t st = (cudaStream_t)stream;
+  if (BN == 128) return mix ? launch_conv<128, 1, true>(tx, tw, a, B, st) : launch_conv<128, 1, false>(tx, tw, a, B, st);
+  return mix ? launch_conv<64, 1, true>(tx, tw, a, B, st) : launch_conv<64, 1, false>(tx, tw, a, B, st);
+}
+
+extern "C" int VSB_API(vsb_vae_time_conv_rgb)(const vsb_bf16* x, const vsb_bf16* w, const vsb_bf16* bias, vsb_bf16* out,
+                                              int B, int T, int H, int W, void* stream) {
+  if (!x || !w || !bias || !out || B <= 0 || T <= 0 || H <= 0 || W <= 0) return fail(VSB_ERR_INVALID, "vae_time_conv_rgb: bad args");
+  const long long P = (long long)H * W;
+  time_conv_rgb_kernel<<<grid_for((long long)B * T * P), 256, 0, (cudaStream_t)stream>>>((const bf16*)x, (const bf16*)w,
+                                                                                         (const bf16*)bias, (bf16*)out, B, T, P);
+  return check_launch("vae_time_conv_rgb");
 }
 
 extern "C" int VSB_API(vsb_vae_groupnorm_stats)(const vsb_bf16* x, float* stats, float* workspace, int B, long long P, int C,

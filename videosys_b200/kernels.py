@@ -276,15 +276,50 @@ def vae_conv3d(x, w_packed, bias, cout, kt, resid=None, round_conv=True):
     return out
 
 
+def vae_conv_time(x, w_packed, bias, cout, kt, resid=None, mix=None, round_conv=True):
+    """(kt, 1, 1) convolution of x [B, kt-1+T, H, W, Cin] (channels-last, the time padding materialised as frames of x);
+    w_packed [Cout, kt, Cin] (pack_conv_weight of a [Cout, Cin, kt, 1, 1] weight); returns [B, T, H, W, cout] = conv +
+    bias [+ resid].  mix = (a, b): instead out = a * resid + b * (resid + conv + bias), each op rounded (the SVD
+    temporal decoder's TemporalResnetBlock sum and AlphaBlender)."""
+    lib, st = _prep(x, w_packed, bias, resid)
+    _bf16(x, "x")
+    _same_dtype(x, w_packed, bias, resid)
+    B, Tin, H, W, Cin = x.shape
+    T = Tin - (kt - 1)
+    if mix is not None and resid is None:
+        raise _lib.VsbError("vae_conv_time: mix needs resid")
+    a, b = (0.0, 0.0) if mix is None else (float(mix[0]), float(mix[1]))
+    out = torch.empty(B, T, H, W, cout, dtype=x.dtype, device=x.device)
+    with _Timed("vae_conv_time", 2 * B * T * H * W * cout * Cin * kt):
+        _lib.check(_fn(lib, "vsb_vae_conv_time", x)(_p(x), _p(w_packed), _p(bias), _p(resid), _p(out), B, T, H, W, Cin, cout, kt,
+                                                    int(mix is not None), a, b, int(bool(round_conv)), st), "vae_conv_time")
+    return out
+
+
+def vae_time_conv_rgb(x, weight, bias):
+    """Conv3d 3 -> 3, kernel (3, 1, 1), padding (1, 0, 0), + bias, of x [B, T, H, W, 3]; weight [3, 3, 3, 1, 1] as stored."""
+    lib, st = _prep(x, weight, bias)
+    _bf16(x, "x")
+    _same_dtype(x, weight, bias)
+    B, T, H, W, Cc = x.shape
+    if Cc != 3 or tuple(weight.shape) != (3, 3, 3, 1, 1):
+        raise _lib.VsbError("vae_time_conv_rgb: needs 3 channels and a [3, 3, 3, 1, 1] weight")
+    out = torch.empty_like(x)
+    with _Timed("vae_time_conv_rgb", 2 * x.numel() * 2):
+        _lib.check(_fn(lib, "vsb_vae_time_conv_rgb", x)(_p(x), _p(weight), _p(bias), _p(out), B, T, H, W, st), "vae_time_conv_rgb")
+    return out
+
+
 def pack_conv_weight(w):
     """[Cout, Cin, (kt,) 3, 3] conv weight -> [Cout_pad, kt*9, Cin_pad] tap-major, Cout and Cin zero padded to multiples
-    of 64 (include/vsb200.h)."""
+    of 64 (include/vsb200.h); a (kt, 1, 1) weight [Cout, Cin, kt, 1, 1] -> [Cout_pad, kt, Cin_pad] likewise."""
     if w.dim() == 4:
         w = w[:, :, None]
     cout, cin, kt = w.shape[0], w.shape[1], w.shape[2]
+    taps = kt * w.shape[3] * w.shape[4]
     cout_pad, cin_pad = -(-cout // 64) * 64, -(-cin // 64) * 64
-    p = torch.zeros(cout_pad, kt * 9, cin_pad, dtype=w.dtype, device=w.device)
-    p[:cout, :, :cin] = w.permute(0, 2, 3, 4, 1).reshape(cout, kt * 9, cin)
+    p = torch.zeros(cout_pad, taps, cin_pad, dtype=w.dtype, device=w.device)
+    p[:cout, :, :cin] = w.permute(0, 2, 3, 4, 1).reshape(cout, taps, cin)
     return p
 
 

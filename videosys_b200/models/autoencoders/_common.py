@@ -40,10 +40,11 @@ def conv_kt(conv):
 
 
 def pack_conv(conv):
-    """Sets ``conv._w`` / ``conv._b``: a 3x3 weight in the layout of vae_conv3d, a 1x1 weight as a [Cout, Cin] GEMM
-    weight.  A bias-free convolution carries a zero bias: 16-bit(conv + 0) is the rounded convolution."""
+    """Sets ``conv._w`` / ``conv._b``: a 3x3 or (kt, 1, 1) weight in the layout of vae_conv3d / vae_conv_time, a 1x1
+    (1x1x1) weight as a [Cout, Cin] GEMM weight.  A bias-free convolution carries a zero bias: 16-bit(conv + 0) is the
+    rounded convolution."""
     w = conv.weight.detach()
-    conv._w = kernels.pack_conv_weight(w) if w.shape[-1] == 3 else w.flatten(1).contiguous()
+    conv._w = w.flatten(1).contiguous() if all(k == 1 for k in w.shape[2:]) else kernels.pack_conv_weight(w)
     conv._b = conv.bias.detach() if conv.bias is not None else torch.zeros(conv.out_channels, dtype=w.dtype, device=w.device)
 
 

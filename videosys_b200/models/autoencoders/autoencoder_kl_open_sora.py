@@ -7,8 +7,8 @@ three stages:
   1. ``z * scale + shift`` (persistent buffers, so a checkpoint's values load over the released ones);
   2. the temporal decoder (``temporal_vae``) per micro-batch of ``micro_z_frame_size`` = 5 latent frames, each chunk on its
      own (no causal state between chunks), with its leading ``time_padding`` frames trimmed;
-  3. the SDXL image decoder (``spatial_vae.module``, diffusers' ``AutoencoderKL`` restated: diffusers' parameter names)
-     on ``micro_batch_size`` frames at a time, each frame its own GroupNorm sample, after ``x / 0.18215``.
+  3. the SDXL image decoder (``spatial_vae.module``, diffusers' ``AutoencoderKL`` of autoencoder_kl.py: diffusers'
+     parameter names) on ``micro_batch_size`` frames at a time, each frame its own GroupNorm sample, after ``x / 0.18215``.
 Activations stay channels-last ``[B, T, H, W, C]`` between kernels:
   - every temporal causal convolution reads a buffer whose kt - 1 = 2 leading context frames are ZEROS (the reference
     pads with ``F.pad(mode="constant")``), followed by the frames the previous kernel wrote there (GroupNorm + SiLU);
@@ -28,10 +28,8 @@ import torch
 import torch.nn as nn
 
 from ... import kernels
-from ._common import (DecoderOnlyVAE, _cast_tuple, attention, check_widths, conv_buffer, conv_kt, group_norm, pad_1x1,
-                      pad_latent, run_conv)
-
-_SILU = 2  # vae_groupnorm_act's F.silu mode
+from ._common import DecoderOnlyVAE, _cast_tuple, check_widths, conv_buffer, conv_kt, group_norm, pad_1x1, pad_latent, run_conv
+from .autoencoder_kl import _SILU, AutoencoderKL
 SCALE = (3.85, 2.32, 2.33, 3.06)  # OpenSoraVAE_V1_2 (:748-749)
 SHIFT = (-0.10, 0.34, 0.27, 0.98)
 SD_SCALING = 0.18215  # VideoAutoencoderKL.decode divides the latent by this (:534)
@@ -177,143 +175,12 @@ def VAE_Temporal_SD(**kwargs):
                         channel_multipliers=(1, 2, 2, 4), temporal_downsample=(False, True, True), **kwargs)
 
 
-# =====================================================================================================================
-# image decoder: diffusers AutoencoderKL (Decoder, UNetMidBlock2D, UpDecoderBlock2D, ResnetBlock2D, Upsample2D,
-# Attention with AttnProcessor2_0), decoder half, with diffusers' parameter names
-# =====================================================================================================================
-class ResnetBlock2D(nn.Module):
-    """norm1 -> SiLU -> conv1 -> norm2 -> SiLU -> conv2, out = (x + h) / 1.0 with x through the 1x1 ``conv_shortcut``
-    (bias) where the width changes.  GroupNorm eps 1e-6."""
-
-    def __init__(self, in_channels, out_channels, groups=32, eps=1e-6):
-        super().__init__()
-        self.in_channels, self.out_channels = in_channels, out_channels
-        self.norm1 = nn.GroupNorm(groups, in_channels, eps=eps)
-        self.conv1 = nn.Conv2d(in_channels, out_channels, 3, padding=1)
-        self.norm2 = nn.GroupNorm(groups, out_channels, eps=eps)
-        self.conv2 = nn.Conv2d(out_channels, out_channels, 3, padding=1)
-        if in_channels != out_channels:
-            self.conv_shortcut = nn.Conv2d(in_channels, out_channels, 1)
-
-    def forward(self, x):
-        h = run_conv(self.conv1, group_norm(self.norm1, x, act=_SILU))
-        n = group_norm(self.norm2, h, act=_SILU)
-        if self.in_channels != self.out_channels:
-            x = kernels.gemm_bias_act(x, self.conv_shortcut._w, self.conv_shortcut._b)
-        return run_conv(self.conv2, n, resid=x)  # dividing by output_scale_factor = 1.0 is exact
-
-
-class Attention(nn.Module):
-    """The mid block's single-head attention (heads = 1, dim_head = C): group_norm, to_q / to_k / to_v, softmax(Q K^T *
-    C^-0.5) V over each frame's pixels, to_out.0, + residual."""
-
-    def __init__(self, channels, groups=32, eps=1e-6):
-        super().__init__()
-        self.group_norm = nn.GroupNorm(groups, channels, eps=eps, affine=True)
-        self.to_q = nn.Linear(channels, channels)
-        self.to_k = nn.Linear(channels, channels)
-        self.to_v = nn.Linear(channels, channels)
-        self.to_out = nn.ModuleList([nn.Linear(channels, channels), nn.Dropout(0.0)])
-        self._w_qkv = self._b_qkv = None
-
-    def pack(self):
-        self._w_qkv = torch.cat([self.to_q.weight, self.to_k.weight, self.to_v.weight]).detach().contiguous()
-        self._b_qkv = torch.cat([self.to_q.bias, self.to_k.bias, self.to_v.bias]).detach().contiguous()
-
-    def forward(self, x):
-        out = self.to_out[0]
-        return attention(x, self.group_norm, self._w_qkv, self._b_qkv, out.weight, out.bias, False)
-
-
-class UNetMidBlock2D(nn.Module):
-    def __init__(self, channels):
-        super().__init__()
-        self.resnets = nn.ModuleList([ResnetBlock2D(channels, channels), ResnetBlock2D(channels, channels)])
-        self.attentions = nn.ModuleList([Attention(channels)])
-
-    def forward(self, x):
-        return self.resnets[1](self.attentions[0](self.resnets[0](x)))
-
-
-class Upsample2D(nn.Module):
-    """Nearest 2x in H and W, then a 3x3 ``conv`` (the fp32 up-cast around the interpolation is exact)."""
-
-    def __init__(self, channels):
-        super().__init__()
-        self.conv = nn.Conv2d(channels, channels, 3, padding=1)
-
-    def forward(self, x):
-        return run_conv(self.conv, kernels.vae_upsample2x(x, False))
-
-
-class UpDecoderBlock2D(nn.Module):
-    def __init__(self, in_channels, out_channels, num_layers, add_upsample):
-        super().__init__()
-        self.resnets = nn.ModuleList([ResnetBlock2D(in_channels if i == 0 else out_channels, out_channels)
-                                      for i in range(num_layers)])
-        self.upsamplers = nn.ModuleList([Upsample2D(out_channels)]) if add_upsample else None
-
-    def forward(self, x):
-        for r in self.resnets:
-            x = r(x)
-        if self.upsamplers is not None:
-            x = self.upsamplers[0](x)
-        return x
-
-
-class SpatialDecoder(nn.Module):
-    """diffusers' ``Decoder``: conv_in, mid_block, up_blocks (widest first, layers_per_block + 1 resnets each, nearest
-    up-sampling after all but the last), conv_norm_out (eps 1e-6) + SiLU, conv_out."""
-
-    def __init__(self, latent_channels=4, out_channels=3, block_out_channels=(128, 256, 512, 512), layers_per_block=2):
-        super().__init__()
-        rev = list(reversed(block_out_channels))
-        self.conv_in = nn.Conv2d(latent_channels, rev[0], 3, padding=1)
-        self.mid_block = UNetMidBlock2D(rev[0])
-        self.up_blocks = nn.ModuleList([])
-        prev = rev[0]
-        for i, ch in enumerate(rev):
-            self.up_blocks.append(UpDecoderBlock2D(prev, ch, layers_per_block + 1, add_upsample=i < len(rev) - 1))
-            prev = ch
-        self.conv_norm_out = nn.GroupNorm(32, block_out_channels[0], eps=1e-6)
-        self.conv_act = nn.SiLU()
-        self.conv_out = nn.Conv2d(block_out_channels[0], out_channels, 3, padding=1)
-
-    def forward(self, z):
-        """z [N, 1, h, w, 16] (frames in the batch, zero padded) -> [N, 1, 8h, 8w, 3]."""
-        x = self.mid_block(run_conv(self.conv_in, z))
-        for up in self.up_blocks:
-            x = up(x)
-        return run_conv(self.conv_out, group_norm(self.conv_norm_out, x, act=_SILU))
-
-
-class AutoencoderKL(nn.Module):
-    """diffusers' AutoencoderKL, decoder half (``post_quant_conv``, ``decoder``).  The SDXL VAE of the released OpenSora
-    v1.2 has block_out_channels (128, 256, 512, 512), layers_per_block 2, latent_channels 4."""
-
-    def __init__(self, block_out_channels: Sequence[int] = (128, 256, 512, 512), layers_per_block: int = 2,
-                 latent_channels: int = 4):
-        super().__init__()
-        self.config = type("Config", (), dict(block_out_channels=tuple(block_out_channels), layers_per_block=layers_per_block,
-                                               latent_channels=latent_channels))()
-        self.post_quant_conv = nn.Conv2d(latent_channels, latent_channels, 1)
-        self.decoder = SpatialDecoder(latent_channels, 3, block_out_channels, layers_per_block)
-        self._pq = None
-
-    def pack(self):
-        self._pq = pad_1x1(self.post_quant_conv.weight, self.post_quant_conv.bias)
-
-    def decode_frames(self, z):
-        """z [N, 1, h, w, 16] -> [N, 1, 8h, 8w, 3]."""
-        return self.decoder(kernels.gemm_bias_act(z, *self._pq))
-
-
 class VideoAutoencoderKL(nn.Module):
     """Reference :488-555, decoder half: frames folded into the batch, ``micro_batch_size`` at a time."""
 
     def __init__(self, micro_batch_size: Optional[int] = 4, block_out_channels: Sequence[int] = (128, 256, 512, 512)):
         super().__init__()
-        self.module = AutoencoderKL(block_out_channels)
+        self.module = AutoencoderKL(block_out_channels=block_out_channels)
         self.out_channels = self.module.config.latent_channels
         self.patch_size = (1, 8, 8)
         self.micro_batch_size = micro_batch_size

@@ -8,8 +8,9 @@ decoder (models/autoencoders/autoencoder_kl_cogvideox.py).  Out of scope as for 
 the LATENTS are returned (``output_type="latent"`` semantics).  dtype follows the reference: fp16 for
 "THUDM/CogVideoX-2b", else bf16.
 
-The video post-processing restates diffusers' ``VideoProcessor.postprocess_video`` (diffusers is not a dependency):
-``(x / 2 + 0.5).clamp(0, 1)`` per frame, then "pt" -> [B, F, 3, H, W], "np" -> [B, F, H, W, 3], "pil" -> lists of PIL images.
+The video post-processing restates diffusers' ``VideoProcessor.postprocess_video`` (pipelines/_common.py, diffusers is not
+a dependency): ``(x / 2 + 0.5).clamp(0, 1)`` per frame, then "pt" -> [B, F, 3, H, W], "np" -> [B, F, H, W, 3], "pil" ->
+lists of PIL images.
 """
 import zlib
 from typing import Callable, Optional
@@ -19,7 +20,7 @@ import torch
 from ...core.pab.pab_mgr import PABConfig, enable_pab, set_pab_manager, update_steps
 from ...models.transformers.cogvideox_transformer_3d import CogVideoXTransformer3DModel
 from ...schedulers.scheduling_ddim_cogvideox import CogVideoXDDIMScheduler
-from .._common import ParallelPipelineMixin
+from .._common import ParallelPipelineMixin, postprocess_frames
 from ..open_sora.pipeline_open_sora import VideoSysPipelineOutput
 
 
@@ -101,17 +102,7 @@ class CogVideoXPipeline(ParallelPipelineMixin):
         z = latents.permute(0, 2, 1, 3, 4)
         z = 1 / self.vae.config.scaling_factor * z
         frames = self.vae.decode(z).sample  # [B, 3, F, H, W]
-        video = (frames / 2 + 0.5).clamp(0, 1).permute(0, 2, 1, 3, 4)  # [B, F, 3, H, W]
-        if output_type == "pt":
-            return video
-        arr = video.permute(0, 1, 3, 4, 2).float().cpu().numpy()  # [B, F, H, W, 3]
-        if output_type == "np":
-            return arr
-        if output_type == "pil":
-            from PIL import Image
-
-            return [[Image.fromarray((f * 255).round().astype("uint8")) for f in clip] for clip in arr]
-        raise ValueError(f"output_type={output_type!r}: expected 'pil', 'np', 'pt' or 'latent'")
+        return postprocess_frames(frames.permute(0, 2, 1, 3, 4), output_type)
 
     def _embeds(self, prompt, negative_prompt, max_sequence_length):
         cfg = self.transformer.config

@@ -3,11 +3,15 @@ VchitectConfig :56-127, VchitectXLPipeline.generate :712-1009) around the native
 
 In scope: the config classes, ``generate()``'s signature, the denoising loop as the reference runs it (:916-954: the
 unconditional and the text branch are two batch-1 forwards, the guidance scale follows the cosine ramp of :943-945,
-flow-match Euler update) and the denoiser.  Out of scope as for the other pipelines (SURVEY.md 2.1): the three text
-encoders and the VAE -- pass ``prompt_embeds`` / ``pooled_prompt_embeds`` (and the negative pair) or a ``text_encoder_fn``;
-without a ``vae_decode_fn`` the LATENTS ``[1, frames, C, H/8, W/8]`` are returned.  dtype bf16 as the reference (:186).
+flow-match Euler update), the denoiser, and -- opt-in through ``VchitectConfig(vae=...)`` -- the VAE decode tail
+(:980-986) on the native image decoder (models/autoencoders/autoencoder_kl.py, the snapshot's ``vae/`` folder, :214-215)
+with diffusers' ``VaeImageProcessor.postprocess`` per frame (pipelines/_common.py).  Out of scope as for the other
+pipelines (SURVEY.md 2.1): the three text encoders -- pass ``prompt_embeds`` / ``pooled_prompt_embeds`` (and the
+negative pair) or a ``text_encoder_fn``.  Without a ``vae`` or a ``vae_decode_fn`` the LATENTS ``[1, frames, C, H/8,
+W/8]`` are returned.  dtype bf16 as the reference (:186).
 """
 import math
+import os
 import zlib
 from typing import Callable, Optional
 
@@ -16,7 +20,8 @@ import torch
 from ...core.pab.pab_mgr import PABConfig, enable_pab, set_pab_manager, update_steps
 from ...models.transformers.vchitect_transformer_3d import VchitectXLTransformerModel
 from ...schedulers.scheduling_flow_match_euler import FlowMatchEulerDiscreteScheduler
-from .._common import ParallelPipelineMixin
+from ...models.autoencoders.autoencoder_kl import AutoencoderKL
+from .._common import ParallelPipelineMixin, decode_image_frames, postprocess_frames
 from ..open_sora.pipeline_open_sora import VideoSysPipelineOutput
 
 
@@ -34,7 +39,7 @@ class VchitectConfig:
     def __init__(self, model_path: str = "Vchitect/Vchitect-2.0-2B", num_gpus: int = 1, cpu_offload: bool = False,
                  enable_pab: bool = False, pab_config=None, transformer_config: Optional[dict] = None, state_dict=None,
                  scheduler_shift: float = 3.0, text_encoder_fn: Optional[Callable] = None,
-                 vae_decode_fn: Optional[Callable] = None):
+                 vae_decode_fn: Optional[Callable] = None, vae=None):
         self.model_path = model_path
         self.pipeline_cls = VchitectXLPipeline
         self.num_gpus = num_gpus
@@ -48,10 +53,13 @@ class VchitectConfig:
         self.scheduler_shift = scheduler_shift
         self.text_encoder_fn = text_encoder_fn
         self.vae_decode_fn = vae_decode_fn
+        # native VAE decoder: a local snapshot root (its vae/ folder is read) or an AutoencoderKL instance
+        self.vae = vae
 
 
 class VchitectXLPipeline(ParallelPipelineMixin):
     vae_scale_factor = 8
+    vae = None  # the native VAE decoder (_load_vae); without one generate returns the latents
 
     def __init__(self, config: VchitectConfig, device=None, dtype: torch.dtype = torch.bfloat16):
         if not torch.cuda.is_available():
@@ -69,9 +77,27 @@ class VchitectXLPipeline(ParallelPipelineMixin):
             self.transformer.load_state_dict(config.state_dict)
         self.transformer = self.transformer.to(self._device).eval()
         self.scheduler = FlowMatchEulerDiscreteScheduler(shift=config.scheduler_shift)
+        self.vae = self._load_vae()
         if config.enable_pab:
             set_pab_manager(config.pab_config)
         self._set_parallel()
+
+    def _load_vae(self):
+        """The native decoder of ``config.vae`` in the pipeline dtype (reference :214-215)."""
+        v = self._config.vae
+        if v is None:
+            return None
+        if not isinstance(v, AutoencoderKL):
+            v = AutoencoderKL.from_pretrained(os.fspath(v), subfolder="vae")
+        return v.to(self._dtype).to(self._device).eval()
+
+    def decode_latents_to_video(self, latents, output_type: str = "pil"):
+        """Reference :980-986 on latents [1, F, C, h, w]: ``[[frame_0, ...]]``, each frame post-processed on its own
+        ("pil": a PIL image, "np": [H, W, 3] float32, "pt": [3, H, W]).  The frames are decoded several per pass: each
+        is its own GroupNorm sample, so the result is the reference's frame-by-frame decode."""
+        latents = (latents / self.vae.config.scaling_factor) + self.vae.config.shift_factor
+        frames = decode_image_frames(self.vae, latents[0])
+        return [list(postprocess_frames(frames, output_type))]
 
     def _embeds(self, prompt, negative_prompt, L=333):
         """Synthetic caption embeddings (77 CLIP + 256 T5 tokens, :498) when no text encoder is supplied."""
@@ -129,6 +155,8 @@ class VchitectXLPipeline(ParallelPipelineMixin):
             lat = self.scheduler.step(noise, t, lat)[0]
         if self._config.vae_decode_fn is not None and output_type != "latents":
             video = self._config.vae_decode_fn(lat)
+        elif self.vae is not None and output_type != "latents":
+            video = self.decode_latents_to_video(lat, output_type)
         else:
-            video = lat.float().cpu()  # latents: the VAE is out of scope
+            video = lat.float().cpu()  # latents
         return VideoSysPipelineOutput(video=video) if return_dict else (video,)
