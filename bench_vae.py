@@ -2,7 +2,7 @@
 of the same modules (the stand-ins of tests/kernels_emul_vae.py, which compute what the reference's eager decoders
 compute), in alternating rounds after a warm-up round.
 
-    python bench_vae.py [--rounds 3] [cogvideox|osp|opensora|latte|vchitect ...]    (all by default)
+    python bench_vae.py [--rounds 3] [cogvideox|osp|opensora|opensora_encode|latte|vchitect ...]    (all by default)
 
 Workloads, random weights:
   - cogvideox: latents [1, 16, 13, 60, 90] (CogVideoX-2b, 49 frames at 480 x 720), fp16, released widths; decoded tiled
@@ -16,13 +16,19 @@ Workloads, random weights:
     the launches of one native decode:
       720p 9:16, 68 frames: latents [1, 4, 20, 90, 160];
       240p 9:16, 51 frames: latents [1, 4, 15, 30, 53].
+  - opensora_encode: bf16, released widths, OpenSoraVAEEncoder.encode with the pipeline's micro-batching (4 images per
+    spatial pass, 17-frame temporal chunks), the posterior noise drawn under one seed in both chains:
+      one 720p 9:16 image (an image-to-video reference): video [1, 3, 1, 720, 1280];
+      a 51-frame 720p clip (a looped generation's re-encode): video [1, 3, 51, 720, 1280];
+      a 51-frame 240p clip: video [1, 3, 51, 240, 426];
+    then the rates of the strided convolution on its own (Downsample2D at the first level, the temporal stride-2 conv).
   - latte: fp16, released widths, latents [1, 4, 16, 64, 64] (16 frames at 512 x 512) as LattePipeline decodes them:
     the SVD temporal decoder on chunks of 14 + 2 frames, and the image VAE (enable_vae_temporal_decoder=False); then the
     rates of the time-axis convolution at the temporal decoder's top level (128 channels, 512 x 512, 14 frames): plain,
     with the residual + AlphaBlender epilogue, and the same result unfused (residual epilogue, then a vae_mix pass).
   - vchitect: bf16, released widths, 16 latent channels, latents [1, 40, 16, 36, 60] (40 frames at 288 x 480), decoded as
     VchitectXLPipeline does (several frames per pass).
-For OpenSora, Latte and Vchitect the FLOPs of the convolutions and GEMMs are counted from the shapes of the launches of
+For OpenSora (decode and encode), Latte and Vchitect the FLOPs of the convolutions and GEMMs are counted from the shapes of the launches of
 one native decode.  Prints the card and its power limit, then one JSON line per model.  For Open-Sora-Plan, OpenSora,
 Latte and Vchitect the decoded frames of the two chains are compared.
 """
@@ -36,10 +42,12 @@ import torch
 
 from oracle import gen_golden_cogvideox_vae as GC, gen_golden_opensora_vae as GS, gen_golden_osp_vae as GP
 from oracle import gen_golden_latte_vae as GL
+from tests import kernels_emul_vae_down as ED
 from tests import kernels_emul_vae_time as EV
 from videosys_b200 import kernels
 from videosys_b200.models.autoencoders import (AutoencoderKL, AutoencoderKLCogVideoX, AutoencoderKLTemporalDecoder,
-                                               CausalVAEModelV110, CausalVAEModelV120, VideoAutoencoderPipeline)
+                                               CausalVAEModelV110, CausalVAEModelV120, OpenSoraVAEEncoder,
+                                               VideoAutoencoderPipeline)
 from videosys_b200.pipelines._common import decode_image_frames
 
 
@@ -55,7 +63,7 @@ def _time(fn):
 @contextlib.contextmanager
 def _eager():
     """The torch stand-ins patched over the kernels for the duration of a with-block."""
-    patch = EV.stand_ins()
+    patch = {**EV.stand_ins(), **ED.stand_ins()}
     saved = {n: getattr(kernels, n) for n in patch}
     for n, f in patch.items():
         setattr(kernels, n, f)
@@ -228,8 +236,8 @@ def opensora(rounds):
 
 # ---- Latte and Vchitect-2.0 ----
 def _flops(decode):
-    """FLOPs of the convolutions and GEMMs of one native decode, from the launches' shapes."""
-    kernels.PROFILE, kernels.PROFILE_KINDS = [], {"vae_conv3d", "vae_conv_time", "gemm"}
+    """FLOPs of the convolutions and GEMMs of one native decode (or encode), from the launches' shapes."""
+    kernels.PROFILE, kernels.PROFILE_KINDS = [], {"vae_conv3d", "vae_conv_time", "vae_conv_down", "gemm"}
     try:
         decode()
         torch.cuda.synchronize()
@@ -300,7 +308,50 @@ def vchitect(rounds):
     return {"workload": "vchitect_vae_decode_1x40x16x36x60_bf16", **_run("vchitect", lambda: decode_image_frames(vae, z[0]), rounds)}
 
 
-MODELS = {"cogvideox": cogvideox, "osp": osp, "opensora": opensora, "latte": latte, "vchitect": vchitect}
+# ---- OpenSora v1.2 encoder ----
+OPENSORA_ENCODE_WORKLOADS = {"720p_image": (1, 3, 1, 720, 1280), "720p_51f": (1, 3, 51, 720, 1280),
+                             "240p_51f": (1, 3, 51, 240, 426)}
+
+
+def conv_down_rates(dt):
+    """ms and TFLOP/s of vae_conv_down at the encoders' shapes."""
+    g = torch.Generator(device="cuda").manual_seed(0)
+    res = {}
+    for name, (N, T, H, W, C, kt) in {"down2d_128_720x1280_n4": (4, 1, 720, 1280, 128, 1),
+                                      "down2d_512_180x320_n4": (4, 1, 180, 320, 512, 1),
+                                      "down_t_256_90x160_t20": (1, 20, 90, 160, 256, 3)}.items():
+        x = torch.randn(N, T, H, W, C, device="cuda", generator=g).to(dt)
+        wp = kernels.pack_conv_weight((0.02 * torch.randn(C, C, kt, 3, 3, device="cuda", generator=g)).to(dt))
+        b = torch.zeros(C, device="cuda", dtype=dt)
+        out = kernels.vae_conv_down(x, wp, b, C, kt)
+        flop = 2 * out.numel() * C * kt * 9
+        ms = _events(lambda: kernels.vae_conv_down(x, wp, b, C, kt), 10)
+        res[name] = {"ms": round(ms, 3), "tflops": round(flop / ms / 1e9, 1)}
+    return res
+
+
+def opensora_encode(rounds):
+    dt = torch.bfloat16
+    enc = OpenSoraVAEEncoder()
+    enc.load_state_dict(GS.weights(enc.state_dict(), "released"))
+    enc = enc.to(dt).cuda().eval()
+
+    def encode(x):
+        torch.manual_seed(0)  # the same posterior noise in both chains
+        return enc.encode(x)
+
+    result = {}
+    for wl, shape in OPENSORA_ENCODE_WORKLOADS.items():
+        x = (2 * torch.rand(*shape, generator=torch.Generator().manual_seed(0)) - 1).to(dt).cuda()
+        result[wl] = _run(f"opensora_encode {wl}", lambda: encode(x), rounds)
+        del x
+        torch.cuda.empty_cache()
+    result["kernels"] = conv_down_rates(dt)
+    return result
+
+
+MODELS = {"cogvideox": cogvideox, "osp": osp, "opensora": opensora, "opensora_encode": opensora_encode, "latte": latte,
+          "vchitect": vchitect}
 
 
 def main():

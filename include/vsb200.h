@@ -261,8 +261,8 @@ int vsb_ipc_close_handle(void* devptr);
  *   padding (:131-132) is not materialised.  w_packed [Cout_pad, kt*9, Cin_pad] is the weight packed tap-major (tap =
  *   (dt*3 + dy)*3 + dx), Cin_pad / Cout_pad = Cin / Cout rounded up to a multiple of 64,
  *   zero padded.  out = bf16(conv + bias) [+ resid, rounded again: the ResNet sum of :298]; round_conv = 1 rounds the
- *   convolution to 16 bits before the bias is added.  Cin = 16 or a multiple of 64; Cout = 3, 4 or a multiple of 64
- *   (4: the OpenSora v1.2 temporal decoder's conv_out).
+ *   convolution to 16 bits before the bias is added.  Cin = 16 or a multiple of 64; Cout = 3, 4, 8 or a multiple of 64
+ *   (4: the OpenSora v1.2 temporal decoder's conv_out; 8: the SDXL image encoder's conv_out).
  * vsb_vae_groupnorm_stats: mean and rstd = rsqrt(var + eps) (fp32, stats [B, G, 2]) of nn.GroupNorm over x [B, P, C]
  *   (P = T*H*W pixels).  workspace: B * VSB_GN_CHUNKS * C * 2 floats.  The sums are shifted by each channel's value at
  *   the sample's first pixel, so a DC offset large against the spread does not cancel the variance away.  Fixed-order
@@ -325,6 +325,23 @@ int vsb_vae_attn_merge(const vsb_bf16* o, vsb_bf16* out, int B, int T, int P, in
  *   movement (bit exact).  C % 8 == 0, 16-byte aligned pointers. */
 int vsb_vae_depth_to_time(const vsb_bf16* x, vsb_bf16* out, int B, int T, int H, int W, int C, int t_off, int T_out,
                           void* stream);
+
+/* ---- OpenSora v1.2 VAE encoder (models/autoencoders/autoencoder_kl_open_sora.py, OpenSoraVAEEncoder) ----------------
+ * The temporal encoder (reference Encoder :177-272) and the SDXL image encoder (diffusers' Encoder) run on the decoder's
+ * entries above (vsb_vae_conv3d with Cout = 8 for the image encoder's conv_out; RGB and the 4-channel latent zero
+ * padded to 16 channels on the host) plus:
+ * vsb_vae_conv_down: the two down-sampling convolutions on the implicit GEMM of vsb_vae_conv3d, x [B, Tin, Hin, Win, Cin]
+ *   -> out [B, T, H, W, Cout] = bf16(conv + bias) (round_conv as in vsb_vae_conv3d), w_packed as for vsb_vae_conv3d:
+ *   - kt = 1, stride_t = 1, stride_hw = 2: Downsample2D, F.pad(x, (0, 1, 0, 1)) then a 3x3 conv with stride 2 (T = Tin,
+ *     H = (Hin - 2) / 2 + 1, W likewise).  The A tile is a TMA box with traversal strides 2 in W and H; the right and
+ *     bottom zero padding is its out-of-bounds fill.  Hin, Win >= 2.
+ *   - kt = 3, stride_t = 2, stride_hw = 1: CausalConv3d(k=3, strides=(2, 1, 1)) (:107-124), whose time_pad is one zero
+ *     frame in front: x holds the Tin real frames only, and output frame t reads frames 2t - 1 .. 2t + 1 of x, frame -1
+ *     being the TMA out-of-bounds zero fill (T = (Tin - 2) / 2 + 1, Tin >= 2).  Spatial zero padding 1 as
+ *     vsb_vae_conv3d.
+ *   Cin = 16 or a multiple of 64; Cout = 8 or a multiple of 64. */
+int vsb_vae_conv_down(const vsb_bf16* x, const vsb_bf16* w_packed, const vsb_bf16* bias, vsb_bf16* out, int B, int Tin,
+                      int Hin, int Win, int Cin, int Cout, int kt, int stride_t, int stride_hw, int round_conv, void* stream);
 
 /* ---- SVD temporal decoder (Latte's vae_temporal_decoder, models/autoencoders/autoencoder_kl_temporal_decoder.py) -----
  * The per-frame ResnetBlock2D halves, the mid-block attention and the up-samplers run on the entries above; the
@@ -424,6 +441,9 @@ int vsb_vae_conv_time_f16(const vsb_f16* x, const vsb_f16* w_packed, const vsb_f
                           int round_conv, void* stream);
 int vsb_vae_time_conv_rgb_f16(const vsb_f16* x, const vsb_f16* w, const vsb_f16* bias, vsb_f16* out, int B, int T, int H,
                               int W, void* stream);
+int vsb_vae_conv_down_f16(const vsb_f16* x, const vsb_f16* w_packed, const vsb_f16* bias, vsb_f16* out, int B, int Tin,
+                          int Hin, int Win, int Cin, int Cout, int kt, int stride_t, int stride_hw, int round_conv,
+                          void* stream);
 
 #ifdef __cplusplus
 }

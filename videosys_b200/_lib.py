@@ -57,6 +57,7 @@ SIGNATURES = {
     "vsb_vae_depth_to_time": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "vsb_vae_conv_time": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _f, _f, _i, _vp]),
     "vsb_vae_time_conv_rgb": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
+    "vsb_vae_conv_down": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "vsb_tmap_cache_stats": (C.c_ulonglong, [_i]),
     "vsb_dsp_alloc": (_i, [C.POINTER(_vp), _sz]),
     "vsb_dsp_free": (_i, [_vp]),
@@ -72,7 +73,8 @@ F16_TWINS = ("vsb_ln_modulate", "vsb_ln_modulate_affine", "vsb_modulation_table"
              "vsb_dwconv_shuffle", "vsb_gate_residual_unshuffle", "vsb_dwconv_ffn", "vsb_kv_compress",
              "vsb_vae_conv3d", "vsb_vae_groupnorm_stats", "vsb_vae_spatial_norm_silu", "vsb_vae_upsample2x",
              "vsb_vae_groupnorm_act", "vsb_vae_upsample_linear2x", "vsb_vae_mix", "vsb_vae_attn_split", "vsb_vae_attn_softmax",
-             "vsb_vae_attn_merge", "vsb_vae_depth_to_time", "vsb_vae_conv_time", "vsb_vae_time_conv_rgb")
+             "vsb_vae_attn_merge", "vsb_vae_depth_to_time", "vsb_vae_conv_time", "vsb_vae_time_conv_rgb",
+             "vsb_vae_conv_down")
 for _n in F16_TWINS:
     SIGNATURES[_n + "_f16"] = SIGNATURES[_n]
 

@@ -41,7 +41,7 @@ static int load_encode() {
 struct TmapKey {
   const void* base;
   unsigned long long dims[5], strides[4];
-  unsigned box[5];
+  unsigned box[5], estr[5];
   int rank, swz;
   int dtype, pad_;
   bool operator==(const TmapKey& o) const { return memcmp(this, &o, sizeof(TmapKey)) == 0; }
@@ -64,11 +64,14 @@ static std::atomic<unsigned long long> g_tmap_hits{0}, g_tmap_misses{0};
 static int g_opt_tmap_cache = 1;
 
 static int make_tmap_bf16_uncached(int dtype, CUtensorMap* m, const void* base, int rank, const unsigned long long* dims,
-                                   const unsigned long long* strides_bytes, const unsigned* box, CUtensorMapSwizzle swz);
+                                   const unsigned long long* strides_bytes, const unsigned* box, CUtensorMapSwizzle swz,
+                                   const unsigned* elem_strides);
 
 int make_tmap_elem(int dtype, CUtensorMap* m, const void* base, int rank, const unsigned long long* dims,
-                   const unsigned long long* strides_bytes, const unsigned* box, CUtensorMapSwizzle swz) {
-  if (!g_opt_tmap_cache || rank < 1 || rank > 5) return make_tmap_bf16_uncached(dtype, m, base, rank, dims, strides_bytes, box, swz);
+                   const unsigned long long* strides_bytes, const unsigned* box, CUtensorMapSwizzle swz,
+                   const unsigned* elem_strides) {
+  if (!g_opt_tmap_cache || rank < 1 || rank > 5)
+    return make_tmap_bf16_uncached(dtype, m, base, rank, dims, strides_bytes, box, swz, elem_strides);
   TmapKey key;
   memset(&key, 0, sizeof(key));
   key.base = base;
@@ -78,6 +81,7 @@ int make_tmap_elem(int dtype, CUtensorMap* m, const void* base, int rank, const 
   for (int i = 0; i < rank; ++i) {
     key.dims[i] = dims[i];
     key.box[i] = box[i];
+    key.estr[i] = elem_strides ? elem_strides[i] : 1;
     if (i > 0) key.strides[i - 1] = strides_bytes[i - 1];
   }
   {
@@ -89,7 +93,7 @@ int make_tmap_elem(int dtype, CUtensorMap* m, const void* base, int rank, const 
       return VSB_OK;
     }
   }
-  int rc = make_tmap_bf16_uncached(dtype, m, base, rank, dims, strides_bytes, box, swz);
+  int rc = make_tmap_bf16_uncached(dtype, m, base, rank, dims, strides_bytes, box, swz, elem_strides);
   if (rc) return rc;
   g_tmap_misses.fetch_add(1, std::memory_order_relaxed);
   std::lock_guard<std::mutex> g(g_tmap_mu);
@@ -99,7 +103,8 @@ int make_tmap_elem(int dtype, CUtensorMap* m, const void* base, int rank, const 
 }
 
 static int make_tmap_bf16_uncached(int dtype, CUtensorMap* m, const void* base, int rank, const unsigned long long* dims,
-                                   const unsigned long long* strides_bytes, const unsigned* box, CUtensorMapSwizzle swz) {
+                                   const unsigned long long* strides_bytes, const unsigned* box, CUtensorMapSwizzle swz,
+                                   const unsigned* elem_strides) {
   int rc = load_encode();
   if (rc) return rc;
   cuuint64_t gdim[5];
@@ -108,7 +113,7 @@ static int make_tmap_bf16_uncached(int dtype, CUtensorMap* m, const void* base, 
   for (int i = 0; i < rank; ++i) {
     gdim[i] = dims[i];
     bdim[i] = box[i];
-    estr[i] = 1;
+    estr[i] = elem_strides ? elem_strides[i] : 1;
     if (i > 0) {
       gstr[i - 1] = strides_bytes[i - 1];
       if (gstr[i - 1] % 16) return fail(VSB_ERR_UNSUPPORTED, "tensor map stride %llu not a multiple of 16 bytes", (unsigned long long)gstr[i - 1]);

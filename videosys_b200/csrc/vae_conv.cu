@@ -17,6 +17,11 @@
 // TAPS is the number of spatial taps per frame: 9 for the (kt, 3, 3) convolutions, 1 for the (kt, 1, 1) time-axis
 // convolution of the SVD temporal decoder (vsb_vae_conv_time), where only the A box's frame coordinate moves per tap.
 // MIX adds that decoder's residual and AlphaBlender to the epilogue (see vsb_vae_conv_time).
+// SHW / ST are the spatial and temporal strides of the down-sampling convolutions of the OpenSora v1.2 VAE encoder
+// (vsb_vae_conv_down).  SHW = 2: the A box is a 5-D TMA box with traversal strides {1, 2, 2, 1, 1} over 64 x 32 x 16
+// input elements, which lands the same 128 x 64 K-major tile; the taps start at (2 w0 + dx, 2 h0 + dy), dx, dy in
+// {0, 1, 2}, and the (0, 1, 0, 1) zero padding of Downsample2D is the out-of-bounds fill.  ST = 2: output frame t reads
+// input frames 2t - 1 .. 2t + 1; the causal time pad (one zero frame in front) is the out-of-bounds fill of frame -1.
 #include "vsb_common.cuh"
 #include "vsb_host.h"
 #include "wgmma.cuh"
@@ -54,10 +59,11 @@ struct ConvArgs {
   float mix_a, mix_b;  // MIX only: the AlphaBlender's weights of resid and of resid + conv
 };
 
-template <int BN, int TAPS = 9, bool MIX = false>
+template <int BN, int TAPS = 9, bool MIX = false, int SHW = 1, int ST = 1>
 __global__ void __launch_bounds__(kConvThreads, 1)
 vae_conv_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_w, const ConvArgs a) {
   static_assert(TAPS == 9 || TAPS == 1, "3x3 or 1x1 spatial taps");
+  static_assert((SHW == 1 || (SHW == 2 && TAPS == 9)) && (ST == 1 || ST == 2), "strides 1 or 2 (spatial: 3x3 taps)");
   using Cfg = ConvCfg<BN>;
   extern __shared__ unsigned char smem_dyn[];
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~uintptr_t(1023));
@@ -92,13 +98,15 @@ vae_conv_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant_
     if (threadIdx.x == 0) {
       int kb = 0;
       for (int tap = 0; tap < taps; ++tap) {
-        const int dz = tap / TAPS, dy = TAPS == 9 ? (tap / 3) % 3 - 1 : 0, dx = TAPS == 9 ? tap % 3 - 1 : 0;
+        // stride 1: centred taps (-1, 0, 1); stride 2: the padding is on the far side only, taps (0, 1, 2)
+        constexpr int kLead = SHW == 1 ? 1 : 0;
+        const int dz = tap / TAPS, dy = TAPS == 9 ? (tap / 3) % 3 - kLead : 0, dx = TAPS == 9 ? tap % 3 - kLead : 0;
         for (int cs = 0; cs < a.cin_slices; ++cs, ++kb) {
           const int s = kb % kConvStages;
           mbar_wait_quiet(&empty[s], ((kb / kConvStages) & 1) ^ 1);
           unsigned char* st = smem + s * Cfg::kStageBytes;
           mbar_arrive_expect_tx(&full[s], Cfg::kStageBytes);
-          tma_load_5d(&tm_x, &full[s], st, cs * kConvBK, w0 + dx, h0 + dy, t + dz, b);
+          tma_load_5d(&tm_x, &full[s], st, cs * kConvBK, SHW * w0 + dx, SHW * h0 + dy, ST * t + dz - (ST - 1), b);
           tma_load_2d(&tm_w, &full[s], st + Cfg::kABytes, (tap * a.cin_slices + cs) * kConvBK, n0);
         }
       }
@@ -172,19 +180,19 @@ vae_conv_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant_
   }
 }
 
-template <int BN, int TAPS = 9, bool MIX = false>
+template <int BN, int TAPS = 9, bool MIX = false, int SHW = 1, int ST = 1>
 int launch_conv(const CUtensorMap& tx, const CUtensorMap& tw, const ConvArgs& a, int B, cudaStream_t st) {
-  const char* what = TAPS == 9 ? "vae_conv3d" : "vae_conv_time";
+  const char* what = SHW * ST > 1 ? "vae_conv_down" : TAPS == 9 ? "vae_conv3d" : "vae_conv_time";
   static bool attr = false;
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(vae_conv_kernel<BN, TAPS, MIX>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = cudaFuncSetAttribute(vae_conv_kernel<BN, TAPS, MIX, SHW, ST>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          ConvCfg<BN>::kSmemBytes);
     if (e != cudaSuccess) return fail(VSB_ERR_CUDA, "%s: smem attr: %s", what, cudaGetErrorString(e));
     attr = true;
   }
   const long long tiles = (long long)B * a.T * a.tiles_h * a.tiles_w * a.tiles_n;
   if (tiles >= (1ll << 31)) return fail(VSB_ERR_UNSUPPORTED, "%s: too many tiles", what);
-  vae_conv_kernel<BN, TAPS, MIX><<<(unsigned)tiles, kConvThreads, ConvCfg<BN>::kSmemBytes, st>>>(tx, tw, a);
+  vae_conv_kernel<BN, TAPS, MIX, SHW, ST><<<(unsigned)tiles, kConvThreads, ConvCfg<BN>::kSmemBytes, st>>>(tx, tw, a);
   return check_launch(what);
 }
 
@@ -427,15 +435,17 @@ using namespace vsb;
 namespace vsb {
 namespace {
 // The two TMA operands of vae_conv_kernel: x [B, Tin, H, W, Cin] as 64-channel x 16 x 8 x 1 x 1 boxes and the packed
-// weight [Cout_pad, K] as 64 x BN boxes, both 128B-swizzled.
+// weight [Cout_pad, K] as 64 x BN boxes, both 128B-swizzled.  shw = 2: the x box spans 32 x 16 pixels traversed with
+// stride 2 in W and H (16 x 8 pixels land).
 int conv_tmaps(CUtensorMap* tx, CUtensorMap* tw, const void* x, const void* w_packed, int B, int Tin, int H, int W, int Cin,
-               unsigned long long K, int cout_pad, int BN) {
+               unsigned long long K, int cout_pad, int BN, int shw = 1) {
   unsigned long long dx[5] = {(unsigned long long)Cin, (unsigned long long)W, (unsigned long long)H, (unsigned long long)Tin,
                               (unsigned long long)B};
   unsigned long long sx[4] = {(unsigned long long)Cin * 2, (unsigned long long)W * Cin * 2,
                               (unsigned long long)H * W * Cin * 2, (unsigned long long)Tin * H * W * Cin * 2};
-  unsigned bx[5] = {kConvBK, kConvBW, kConvBH, 1, 1};
-  int rc = make_tmap_bf16(tx, x, 5, dx, sx, bx, CU_TENSOR_MAP_SWIZZLE_128B);
+  unsigned bx[5] = {kConvBK, (unsigned)(kConvBW * shw), (unsigned)(kConvBH * shw), 1, 1};
+  unsigned ex[5] = {1, (unsigned)shw, (unsigned)shw, 1, 1};
+  int rc = make_tmap_bf16(tx, x, 5, dx, sx, bx, CU_TENSOR_MAP_SWIZZLE_128B, ex);
   if (rc) return rc;
   unsigned long long dw[2] = {K, (unsigned long long)cout_pad};
   unsigned long long sw[1] = {K * 2};
@@ -452,8 +462,8 @@ extern "C" int VSB_API(vsb_vae_conv3d)(const vsb_bf16* x, const vsb_bf16* w_pack
     return fail(VSB_ERR_INVALID, "vae_conv3d: bad args");
   if (kt != 1 && kt != 3) return fail(VSB_ERR_UNSUPPORTED, "vae_conv3d: kt=%d (need 1 or 3)", kt);
   if (!(Cin == 16 || Cin % 64 == 0)) return fail(VSB_ERR_UNSUPPORTED, "vae_conv3d: Cin=%d (need 16 or a multiple of 64)", Cin);
-  if (!(Cout == 3 || Cout == 4 || Cout % 64 == 0))
-    return fail(VSB_ERR_UNSUPPORTED, "vae_conv3d: Cout=%d (need 3, 4 or a multiple of 64)", Cout);
+  if (!(Cout == 3 || Cout == 4 || Cout == 8 || Cout % 64 == 0))
+    return fail(VSB_ERR_UNSUPPORTED, "vae_conv3d: Cout=%d (need 3, 4, 8 or a multiple of 64)", Cout);
   if (!aligned16(x) || !aligned16(w_packed) || (resid && ((uintptr_t)resid & 3)) || ((uintptr_t)out & 3))
     return fail(VSB_ERR_UNSUPPORTED, "vae_conv3d: misaligned pointer");
   const int BN = Cout % 128 == 0 ? 128 : 64;
@@ -486,6 +496,37 @@ extern "C" int VSB_API(vsb_vae_conv_time)(const vsb_bf16* x, const vsb_bf16* w_p
   cudaStream_t st = (cudaStream_t)stream;
   if (BN == 128) return mix ? launch_conv<128, 1, true>(tx, tw, a, B, st) : launch_conv<128, 1, false>(tx, tw, a, B, st);
   return mix ? launch_conv<64, 1, true>(tx, tw, a, B, st) : launch_conv<64, 1, false>(tx, tw, a, B, st);
+}
+
+extern "C" int VSB_API(vsb_vae_conv_down)(const vsb_bf16* x, const vsb_bf16* w_packed, const vsb_bf16* bias, vsb_bf16* out,
+                                          int B, int Tin, int Hin, int Win, int Cin, int Cout, int kt, int stride_t,
+                                          int stride_hw, int round_conv, void* stream) {
+  if (!x || !w_packed || !bias || !out || B <= 0 || Tin <= 0 || Hin <= 0 || Win <= 0 || Cin <= 0 || Cout <= 0)
+    return fail(VSB_ERR_INVALID, "vae_conv_down: bad args");
+  const bool spatial = kt == 1 && stride_t == 1 && stride_hw == 2, temporal = kt == 3 && stride_t == 2 && stride_hw == 1;
+  if (!spatial && !temporal)
+    return fail(VSB_ERR_UNSUPPORTED, "vae_conv_down: kt=%d strides (%d, %d) (need kt 1 / (1, 2) or kt 3 / (2, 1))", kt,
+                stride_t, stride_hw);
+  if ((spatial && (Hin < 2 || Win < 2)) || (temporal && Tin < 2))
+    return fail(VSB_ERR_INVALID, "vae_conv_down: input %dx%dx%d smaller than the padded kernel", Tin, Hin, Win);
+  if (!(Cin == 16 || Cin % 64 == 0)) return fail(VSB_ERR_UNSUPPORTED, "vae_conv_down: Cin=%d (need 16 or a multiple of 64)", Cin);
+  if (!(Cout == 8 || Cout % 64 == 0)) return fail(VSB_ERR_UNSUPPORTED, "vae_conv_down: Cout=%d (need 8 or a multiple of 64)", Cout);
+  if (!aligned16(x) || !aligned16(w_packed) || ((uintptr_t)out & 3))
+    return fail(VSB_ERR_UNSUPPORTED, "vae_conv_down: misaligned pointer");
+  // F.pad(x, (0, 1, 0, 1)) then a stride-2 3x3 conv: floor((H + 1 - 3) / 2) + 1; the causal time conv over 1 + Tin
+  // frames: floor((Tin + 1 - 3) / 2) + 1
+  const int T = temporal ? (Tin - 2) / 2 + 1 : Tin, H = spatial ? (Hin - 2) / 2 + 1 : Hin, W = spatial ? (Win - 2) / 2 + 1 : Win;
+  const int BN = Cout % 128 == 0 ? 128 : 64;
+  const int cin_pad = (Cin + 63) / 64 * 64, cout_pad = (Cout + BN - 1) / BN * BN;
+  CUtensorMap tx, tw;
+  int rc = conv_tmaps(&tx, &tw, x, w_packed, B, Tin, Hin, Win, Cin, (unsigned long long)kt * 9 * cin_pad, cout_pad, BN,
+                      stride_hw);
+  if (rc) return rc;
+  ConvArgs a{(const bf16*)bias, nullptr, (bf16*)out, T, H, W, Cout, kt, cin_pad / 64,
+             (H + kConvBH - 1) / kConvBH, (W + kConvBW - 1) / kConvBW, cout_pad / BN, round_conv ? 1 : 0, 0.f, 0.f};
+  cudaStream_t st = (cudaStream_t)stream;
+  if (spatial) return BN == 128 ? launch_conv<128, 9, false, 2, 1>(tx, tw, a, B, st) : launch_conv<64, 9, false, 2, 1>(tx, tw, a, B, st);
+  return BN == 128 ? launch_conv<128, 9, false, 1, 2>(tx, tw, a, B, st) : launch_conv<64, 9, false, 1, 2>(tx, tw, a, B, st);
 }
 
 extern "C" int VSB_API(vsb_vae_time_conv_rgb)(const vsb_bf16* x, const vsb_bf16* w, const vsb_bf16* bias, vsb_bf16* out,

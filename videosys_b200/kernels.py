@@ -296,6 +296,28 @@ def vae_conv_time(x, w_packed, bias, cout, kt, resid=None, mix=None, round_conv=
     return out
 
 
+def vae_conv_down(x, w_packed, bias, cout, kt, round_conv=True):
+    """The OpenSora v1.2 VAE encoder's down-sampling convolutions of x [B, Tin, Hin, Win, Cin] (channels-last), w_packed
+    as for vae_conv3d; returns conv + bias.  kt = 1: Downsample2D (zero pad right and bottom by 1, 3x3 conv, stride 2 in
+    H and W) -> [B, Tin, (Hin - 2) // 2 + 1, (Win - 2) // 2 + 1, cout].  kt = 3: the causal (3, 3, 3) conv with stride
+    (2, 1, 1) and one zero frame in front (not materialised) -> [B, (Tin - 2) // 2 + 1, Hin, Win, cout]."""
+    lib, st = _prep(x, w_packed, bias)
+    _bf16(x, "x")
+    _same_dtype(x, w_packed, bias)
+    B, Tin, Hin, Win, Cin = x.shape
+    if kt == 1:
+        stride_t, stride_hw, T, H, W = 1, 2, Tin, (Hin - 2) // 2 + 1, (Win - 2) // 2 + 1
+    elif kt == 3:
+        stride_t, stride_hw, T, H, W = 2, 1, (Tin - 2) // 2 + 1, Hin, Win
+    else:
+        raise _lib.VsbError(f"vae_conv_down: kt={kt} (need 1: spatial stride 2, or 3: temporal stride 2)")
+    out = torch.empty(B, max(T, 1), max(H, 1), max(W, 1), cout, dtype=x.dtype, device=x.device)
+    with _Timed("vae_conv_down", 2 * out.numel() * Cin * kt * 9):
+        _lib.check(_fn(lib, "vsb_vae_conv_down", x)(_p(x), _p(w_packed), _p(bias), _p(out), B, Tin, Hin, Win, Cin, cout, kt,
+                                                    stride_t, stride_hw, int(bool(round_conv)), st), "vae_conv_down")
+    return out
+
+
 def vae_time_conv_rgb(x, weight, bias):
     """Conv3d 3 -> 3, kernel (3, 1, 1), padding (1, 0, 0), + bias, of x [B, T, H, W, 3]; weight [3, 3, 3, 1, 1] as stored."""
     lib, st = _prep(x, weight, bias)

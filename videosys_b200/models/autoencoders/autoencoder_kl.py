@@ -4,7 +4,9 @@ mid-block ``Attention`` with ``AttnProcessor2_0``) on the sm_90a kernels of csrc
 names.  The image VAE of OpenSora v1.2 (SDXL), of Latte without the temporal decoder (sd-vae-ft-ema) and of
 Vchitect-2.0 (16 latent channels, no ``post_quant_conv``, a ``shift_factor``).
 
-Only the decoder is in scope: ``encode`` raises ``NotImplementedError``.  Images are channels-last ``[N, 1, H, W, C]``
+``AutoencoderKL`` is the decoder half only: its ``encode`` raises ``NotImplementedError``.  The encoder half's blocks
+(``SpatialEncoder``: diffusers' ``Encoder``, ``DownEncoderBlock2D`` and ``Downsample2D`` on the strided vae_conv_down)
+serve the OpenSora v1.2 encoder (autoencoder_kl_open_sora.OpenSoraVAEEncoder).  Images are channels-last ``[N, 1, H, W, C]``
 between kernels (T = 1, so each image is its own GroupNorm sample and the 3x3 convolutions are kt = 1); the latent is
 zero padded to 16 channels; ``post_quant_conv`` and the 1x1 shortcuts are GEMMs on the pixel rows; the mid-block
 attention is one GEMM for q | k | v, the materialised per-image softmax, and ``to_out`` with the residual in the GEMM
@@ -132,6 +134,58 @@ class SpatialDecoder(nn.Module):
         for up in self.up_blocks:
             x = up(x)
         return run_conv(self.conv_out, group_norm(self.conv_norm_out, x, act=_SILU))
+
+
+class Downsample2D(nn.Module):
+    """diffusers' Downsample2D with use_conv and padding 0: F.pad(x, (0, 1, 0, 1)), then a 3x3 ``conv`` with stride 2
+    (vae_conv_down, the padding being its out-of-bounds fill)."""
+
+    def __init__(self, channels):
+        super().__init__()
+        self.conv = nn.Conv2d(channels, channels, 3, stride=2, padding=0)
+
+    def forward(self, x):
+        return kernels.vae_conv_down(x, self.conv._w, self.conv._b, self.conv.out_channels, 1)
+
+
+class DownEncoderBlock2D(nn.Module):
+    def __init__(self, in_channels, out_channels, num_layers, add_downsample):
+        super().__init__()
+        self.resnets = nn.ModuleList([ResnetBlock2D(in_channels if i == 0 else out_channels, out_channels)
+                                      for i in range(num_layers)])
+        self.downsamplers = nn.ModuleList([Downsample2D(out_channels)]) if add_downsample else None
+
+    def forward(self, x):
+        for r in self.resnets:
+            x = r(x)
+        if self.downsamplers is not None:
+            x = self.downsamplers[0](x)
+        return x
+
+
+class SpatialEncoder(nn.Module):
+    """diffusers' ``Encoder`` (double_z): conv_in, down_blocks (layers_per_block resnets each, a stride-2 down-sampling
+    after all but the last), mid_block, conv_norm_out (eps 1e-6) + SiLU, conv_out to 2 * latent_channels."""
+
+    def __init__(self, in_channels=3, latent_channels=4, block_out_channels=(128, 256, 512, 512), layers_per_block=2):
+        super().__init__()
+        self.conv_in = nn.Conv2d(in_channels, block_out_channels[0], 3, padding=1)
+        self.down_blocks = nn.ModuleList([])
+        prev = block_out_channels[0]
+        for i, ch in enumerate(block_out_channels):
+            self.down_blocks.append(DownEncoderBlock2D(prev, ch, layers_per_block, add_downsample=i < len(block_out_channels) - 1))
+            prev = ch
+        self.mid_block = UNetMidBlock2D(prev)
+        self.conv_norm_out = nn.GroupNorm(32, prev, eps=1e-6)
+        self.conv_act = nn.SiLU()
+        self.conv_out = nn.Conv2d(prev, 2 * latent_channels, 3, padding=1)
+
+    def forward(self, x):
+        """x [N, 1, H, W, 16] (images in the batch, RGB zero padded) -> moments [N, 1, h, w, 2 * latent_channels]."""
+        x = run_conv(self.conv_in, x)
+        for down in self.down_blocks:
+            x = down(x)
+        return run_conv(self.conv_out, group_norm(self.conv_norm_out, self.mid_block(x), act=_SILU))
 
 
 class AutoencoderKL(DecoderOnlyVAE):

@@ -1,16 +1,30 @@
 """OpenSora pipeline surface (mirror of videosys/pipelines/open_sora/pipeline_open_sora.py: OpenSoraPABConfig :32-69,
 OpenSoraConfig :126-163, OpenSoraPipeline.generate :426-656) around the native STDiT3.
 
-In scope: the config classes, ``generate()``'s signature, the shape tables, the RFLOW loop and the denoiser, and the VAE
-decode on the native OpenSora v1.2 decoder (models/autoencoders/autoencoder_kl_open_sora.py).  Out of scope (SURVEY.md 2.1
-row 7): the T5 text encoder and prompt cleaning -- pass a ``text_encoder_fn``; without it ``generate`` feeds a
-deterministic synthetic caption embedding.
+In scope: the config classes, ``generate()``'s signature, the shape tables, the RFLOW loop and the denoiser, the VAE
+decode on the native OpenSora v1.2 decoder (models/autoencoders/autoencoder_kl_open_sora.py), and the reference's
+conditioning: image references (``refs``), mask strategies (``ms``) and looped generation (``loop``), on the native
+encoder (conditioning.py).  Out of scope (SURVEY.md 2.1 row 7): the T5 text encoder, prompt cleaning and the aes / flow /
+camera_motion score suffixes -- pass a ``text_encoder_fn``; without it ``generate`` feeds a deterministic synthetic
+caption embedding.
 
 The decode is opt-in: ``OpenSoraConfig(vae=<local snapshot directory or VideoAutoencoderPipeline instance>)`` makes
 ``generate`` return the reference's uint8 video ``[B, T, H, W, 3]`` (:638-648).  The default ``vae`` is the hub id
 "hpcai-tech/OpenSora-VAE-v1.2", which is not a local directory, so by default ``generate`` returns the denoised LATENTS
 exactly as before (the quantity the metric is defined on).  A ``vae_decode_fn`` takes precedence over both.  Under
-sequence parallelism every rank decodes the whole video, as the reference does.
+sequence parallelism every rank decodes the whole video, and encodes its own references with the broadcast seed, as the
+reference does.
+
+Conditioning (``refs``, ``ms`` or ``loop > 1``) needs the native decoder and the native encoder
+(``OpenSoraConfig(vae_encoder=<snapshot directory or OpenSoraVAEEncoder>)``, by default the ``vae`` directory), loaded on
+the first ``generate`` that conditions; without them it raises ValueError.  It follows the reference's order (:519-643):
+the prompt's JSON, every reference encoded, the loop prompts, then per loop the previous clip re-encoded and appended as a
+reference (loop > 0), z drawn, the mask strategies applied, RFLOW with the mask, the decode.
+
+Deliberate deviation: the reference trims and joins the loop clips along dim 1 of ``[B, C, T, H, W]`` (:641-643), the
+channel axis, so ``[:, 17:]`` of 3 channels is empty and it returns only the first clip.  Here each later clip loses its
+first ``dframe_to_frame(condition_frame_length)`` frames and the clips join along TIME (upstream Open-Sora's per-sample
+``[:, dframe_to_frame(cfl):]`` on ``[C, T, H, W]``): ``nf + (loop - 1) * (nf - dframe_to_frame(cfl))`` frames.
 """
 import zlib
 from dataclasses import dataclass
@@ -21,6 +35,7 @@ import torch
 from ...core.pab.pab_mgr import PABConfig, set_pab_manager, update_steps
 from ...models.transformers.open_sora_transformer_3d import STDiT3, STDiT3Config
 from ...schedulers.scheduling_rflow_open_sora import RFLOW
+from . import conditioning as C
 
 # 9:16 ("0.56") and 1:1 base sizes of pipelines/open_sora/data_process.py:63-235; other ratios are not tabulated here
 _IMAGE_SIZE = {
@@ -78,11 +93,15 @@ class OpenSoraConfig:
                  cfg_scale: float = 7.0, cpu_offload: bool = False, tiling_size: int = 4,
                  enable_flash_attn: bool = False, enable_pab: bool = False, pab_config=None,
                  transformer_config: Optional[STDiT3Config] = None, state_dict=None,
-                 text_encoder_fn: Optional[Callable] = None, vae_decode_fn: Optional[Callable] = None):
+                 text_encoder_fn: Optional[Callable] = None, vae_decode_fn: Optional[Callable] = None,
+                 vae_encoder=None):
         self.pipeline_cls = OpenSoraPipeline
         # vae: a local snapshot directory of hpcai-tech/OpenSora-VAE-v1.2 or a VideoAutoencoderPipeline instance decodes
         # natively; anything else (the default hub id) leaves generate() returning latents
         self.transformer, self.vae, self.text_encoder = transformer, vae, text_encoder
+        # vae_encoder: a local snapshot directory or an OpenSoraVAEEncoder instance for refs / ms / loop; None: the vae
+        # directory when vae is one
+        self.vae_encoder = vae_encoder
         self.num_gpus = num_gpus
         self.num_sampling_steps = num_sampling_steps
         self.cfg_scale = cfg_scale
@@ -123,6 +142,7 @@ class OpenSoraPipeline:
         self.scheduler = RFLOW(num_sampling_steps=config.num_sampling_steps, cfg_scale=config.cfg_scale,
                                use_timestep_transform=True)
         self.vae = self._load_vae()
+        self._vae_encoder = None  # loaded by the first generate that conditions
         if config.enable_pab:
             set_pab_manager(config.pab_config)
         self._set_parallel()
@@ -136,14 +156,38 @@ class OpenSoraPipeline:
         vae = load_vae(self._config.vae, micro_batch_size=self._config.tiling_size)
         return None if vae is None else vae.to(torch.bfloat16).to(self._device).eval()
 
+    def _load_vae_encoder(self):
+        """The native encoder for conditioning, in bf16 on the pipeline's device (loaded once), or None."""
+        if self._vae_encoder is None:
+            from ...models.autoencoders.autoencoder_kl_open_sora import load_vae_encoder
+
+            enc = load_vae_encoder(self._config.vae_encoder, self._config.vae, micro_batch_size=self._config.tiling_size)
+            self._vae_encoder = None if enc is None else enc.to(torch.bfloat16).to(self._device).eval()
+        return self._vae_encoder
+
     def decode_latents(self, samples, num_frames: int):
         """The reference tail (:638-648): vae(samples, decode_only=True, num_frames), then clamp_(-1, 1), sub_(-1),
         div_(2), mul(255), add_(0.5), clamp_(0, 255) in bf16, as uint8 [B, T, H, W, 3] on the CPU."""
-        video = self.vae.decode(samples.to(torch.bfloat16), num_frames=num_frames)
+        return self._to_uint8(self.vae.decode(samples.to(torch.bfloat16), num_frames=num_frames))
+
+    @staticmethod
+    def _to_uint8(video):
         low, high = -1, 1
         video.clamp_(min=low, max=high)
         video.sub_(low).div_(max(high - low, 1e-5))
         return video.mul(255).add_(0.5).clamp_(0, 255).permute(0, 2, 3, 4, 1).to("cpu", torch.uint8)
+
+    def _check_conditioning(self, loop, condition_frame_length):
+        """refs / ms / loop need the native decoder and encoder (the decoded clips are re-encoded); raises ValueError."""
+        if loop < 1:
+            raise ValueError(f"loop={loop} must be >= 1")
+        if self._config.vae_decode_fn is not None:
+            raise ValueError("refs / ms / loop decode and re-encode on the native VAE: do not pass vae_decode_fn")
+        if getattr(self, "vae", None) is None or self._load_vae_encoder() is None:
+            raise ValueError("refs / ms / loop need the native OpenSora v1.2 VAE: OpenSoraConfig(vae=<local snapshot "
+                             "directory or VideoAutoencoderPipeline>, vae_encoder=<directory or OpenSoraVAEEncoder>)")
+        if loop > 1:
+            C.dframe_to_frame(condition_frame_length)
 
     def _set_parallel(self, dp_size=None, sp_size=None, enable_cp=False):
         import torch.distributed as dist
@@ -194,8 +238,10 @@ class OpenSoraPipeline:
                  refs: Optional[str] = "", aes: float = 6.5, flow: Optional[float] = None,
                  camera_motion: Optional[float] = None, condition_frame_length: int = 5, align: int = 5,
                  condition_frame_edit: float = 0.0, return_dict: bool = True, verbose: bool = True):
-        if loop != 1 or refs or ms:
-            raise NotImplementedError("reference conditioning / looping are outside the hot-path scope")
+        prompts, refs_l, ms_l = C.extract_json_from_prompts([prompt], [refs or ""], [ms or ""])
+        conditioned = loop != 1 or bool(refs_l[0]) or bool(ms_l[0])
+        if conditioned:
+            self._check_conditioning(loop, condition_frame_length)
         dev, dtype = self._device, torch.bfloat16
         image_size = get_image_size(resolution, aspect_ratio)
         nf = get_num_frames(num_frames)
@@ -207,19 +253,41 @@ class OpenSoraPipeline:
         update_steps(self._config.num_sampling_steps)
         self.transformer.reset_pab_state()
         self._set_seed(seed)
-        y, mask, y_null = self._encode_text(prompt, negative_prompt)
+        encode = None
+        refs_x = [[]]
+        if conditioned:  # every reference encoded now, before z, as the reference does (:532-535)
+            enc = self._vae_encoder
+            encode = lambda x: enc.encode(x.to(enc.device, enc.dtype))  # noqa: E731
+            refs_x = C.collect_references_batch(refs_l, encode, image_size)
+        texts, loop_idx = C.split_prompt(prompts[0])
+        batch_prompts = [C.merge_prompt(texts, loop_idx)]
         Tl, Hl, Wl = get_latent_size(nf, *image_size)
-        z = torch.randn(1, self.transformer.in_channels, Tl, Hl, Wl, device=dev, dtype=dtype)
-        margs = dict(
-            y=y.to(dev, dtype), mask=mask.to(dev),
-            height=torch.tensor([image_size[0]], device=dev, dtype=dtype),
-            width=torch.tensor([image_size[1]], device=dev, dtype=dtype),
-            num_frames=torch.tensor([nf], device=dev, dtype=dtype),
-            fps=torch.tensor([fps], device=dev, dtype=dtype),
-        )
-        masks = torch.ones(1, Tl, device=dev)  # apply_mask_strategy with ms=[""] returns an all-ones mask (:825-854)
-        samples = self.scheduler.sample(self.transformer, z, margs, y_null.to(dev, dtype), dev, mask=masks, progress=verbose)
-        if self._config.vae_decode_fn is not None:
+        clips = []
+        for loop_i in range(loop):
+            prompt_i = C.extract_prompts_loop(batch_prompts, loop_i)[0]
+            if loop_i > 0:  # the previous clip re-encoded as the next one's first frames (:614-617)
+                refs_x, ms_l = C.append_generated(encode, clips[-1], refs_x, ms_l, loop_i, condition_frame_length,
+                                                  condition_frame_edit)
+            y, mask, y_null = self._encode_text(prompt_i, negative_prompt)  # before z, as without conditioning
+            z = torch.randn(1, self.transformer.in_channels, Tl, Hl, Wl, device=dev, dtype=dtype)
+            margs = dict(
+                y=y.to(dev, dtype), mask=mask.to(dev),
+                height=torch.tensor([image_size[0]], device=dev, dtype=dtype),
+                width=torch.tensor([image_size[1]], device=dev, dtype=dtype),
+                num_frames=torch.tensor([nf], device=dev, dtype=dtype),
+                fps=torch.tensor([fps], device=dev, dtype=dtype),
+            )
+            # ms = "" gives an all-ones mask (:825-854)
+            masks = C.apply_mask_strategy(z, refs_x, ms_l, loop_i, align=align)
+            samples = self.scheduler.sample(self.transformer, z, margs, y_null.to(dev, dtype), dev, mask=masks,
+                                            progress=verbose)
+            if conditioned:
+                clips.append(self.vae.decode(samples.to(dtype), num_frames=nf))
+        if conditioned:
+            # the loop clips join along TIME, each later one without its conditioning frames (module docstring)
+            cut = C.dframe_to_frame(condition_frame_length) if loop > 1 else 0
+            video = self._to_uint8(torch.cat([clips[0]] + [c[:, :, cut:] for c in clips[1:]], dim=2))
+        elif self._config.vae_decode_fn is not None:
             video = self._config.vae_decode_fn(samples, nf)
         elif getattr(self, "vae", None) is not None:
             video = self.decode_latents(samples, nf)
