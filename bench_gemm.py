@@ -19,11 +19,11 @@
     python bench_gemm.py [--iters 20] [--warmup 3] [--rounds 3] [--shapes a,b] [--no-cublas] [--out FILE.json]
 
 Inputs are seeded, so two builds given the same arguments can be compared output for output: every shape prints the
-SHA-256 of the output of one launch on fresh inputs.  Rates are 2 M N K FLOPs over the kernel time from CUDA events
-around --iters back-to-back launches; the median over --rounds is reported.  As a ceiling for comparison the same
-operands also go through torch.nn.functional.linear (cuBLAS, bias only: no gate or residual); the library never calls
-cuBLAS.  The card's name, power limit and SM clock (sampled while the launches run) are part of the result.  Needs a CUDA
-device.  Writes nothing unless --out is given.
+kernel instance the library dispatches it to and the SHA-256 of the output of one launch on fresh inputs.  Rates are
+2 M N K FLOPs over the kernel time from CUDA events around --iters back-to-back launches; the median over --rounds is
+reported.  As a ceiling for comparison the same operands also go through torch.nn.functional.linear (cuBLAS, bias only:
+no gate or residual); the library never calls cuBLAS.  The card's name, power limit and SM clock (sampled while the
+launches run) are part of the result.  Needs a CUDA device.  Writes nothing unless --out is given.
 """
 import argparse
 import hashlib
@@ -124,6 +124,16 @@ def _time(fn, iters, warmup):
     return e0.elapsed_time(e1) / iters, clocks["sm_mhz"]
 
 
+def kernel_of(name):
+    """The kernel instance the library launches for a shape."""
+    from videosys_b200 import kernels
+
+    M, N, K, _, epi = SHAPES[name]
+    if isinstance(epi, tuple):
+        return kernels.gemm_kernel_name(M, N, K, residual=True)
+    return kernels.gemm_kernel_name(M, N, K, act=epi)
+
+
 def run_shape(name, seed, iters, warmup, cublas):
     if not torch.cuda.is_available():
         raise SystemExit(f"bench_gemm.py: {name} needs a CUDA device")
@@ -164,15 +174,16 @@ def main():
         for i, name in enumerate(names):
             m = run_shape(name, a.seed + i, a.iters, a.warmup, not a.no_cublas and r == 0)
             cb = f"  cublas {m['cublas_tflops']:6.1f} TFLOP/s" if "cublas_ms" in m else ""
-            print(f"round {r} {name:11s} {m['ms']:9.4f} ms {m['tflops']:6.1f} TFLOP/s{cb}  sm {m['sm_mhz']} MHz  "
-                  f"sha256 {m['sha256']}", flush=True)
+            print(f"round {r} {name:11s} {kernel_of(name):25s} {m['ms']:9.4f} ms {m['tflops']:6.1f} TFLOP/s{cb}  "
+                  f"sm {m['sm_mhz']} MHz  sha256 {m['sha256']}", flush=True)
             runs.setdefault(name, []).append(m)
     res = dict(gpu=gpu_info(), iters=a.iters, rounds=a.rounds, shapes={})
     for name, ms in runs.items():
         M, N, K = SHAPES[name][:3]
         med = statistics.median(m["ms"] for m in ms)
         shas = sorted({m["sha256"] for m in ms})
-        res["shapes"][name] = dict(M=M, N=N, K=K, ms=med, ms_min=min(m["ms"] for m in ms), ms_max=max(m["ms"] for m in ms),
+        res["shapes"][name] = dict(M=M, N=N, K=K, kernel=kernel_of(name), ms=med, ms_min=min(m["ms"] for m in ms),
+                                   ms_max=max(m["ms"] for m in ms),
                                    tflops=round(2 * M * N * K / (med * 1e-3) / 1e12, 1), sha256=shas[0] if len(shas) == 1 else shas,
                                    cublas_tflops=ms[0].get("cublas_tflops"), sm_mhz=[m["sm_mhz"] for m in ms])
     ks = [(SHAPES[n][2], res["shapes"][n]["ms"]) for n in ("q_linear", "k2304", "k4608") if n in res["shapes"]]

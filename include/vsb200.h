@@ -151,6 +151,11 @@ int vsb_gemm_bias_residual(const vsb_bf16* A, const vsb_bf16* W, const vsb_bf16*
                            vsb_bf16* out, const vsb_bf16* mod, const uint8_t* x_mask, int gate_row, int M, int N, int K,
                            int B, int T, int S, void* stream);
 
+/* Name of the kernel instance the two GEMM entries above launch for a shape, e.g. "gemm_wide_kernel<2>" (the same for
+ * bf16 and fp16): act as in vsb_gemm_bias_act, residual != 0 for vsb_gemm_bias_residual (act 0).  "" for bad arguments.
+ * Benchmarks label their rows with it. */
+const char* vsb_gemm_kernel_name(int M, int N, int K, int act, int residual);
+
 /* ---- flash attention (spatial self-attention and text cross-attention) -------------------------------
  * replaces F.scaled_dot_product_attention at attentions.py:100 and :268 (bool key mask = per-batch key count).
  * q/k/v are strided views: element (b, n, h, d) at base + b*batch_stride + n*row_stride + h*D + d (strides in

@@ -28,6 +28,7 @@ SIGNATURES = {
     "vsb_attn_short": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _ll, _ll, _ll, _i, _i, _i, _f, _f, _i, _vp]),
     "vsb_gemm_bias_act": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "vsb_gemm_bias_residual": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "vsb_gemm_kernel_name": (C.c_char_p, [_i, _i, _i, _i, _i]),
     "vsb_attn_flash": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _ll, _ll, _ll, _ll, C.POINTER(_i), _f, _vp]),
     "vsb_pab_gate": (_i, [_i, _i, _i, C.POINTER(_i), _i, _i, _i, _i]),
     "vsb_dsp_wait": (_i, [_vp, _i, _u, _vp]),

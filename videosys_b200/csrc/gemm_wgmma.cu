@@ -1,9 +1,11 @@
 // vsb200 -- 16-bit TN GEMM on the Hopper warpgroup tensor cores: out[M,N] = act(A[M,K] @ W[N,K]^T + bias), or with the
 // residual branch fused into the epilogue: out = resid + [gate *] (A @ W^T + bias).
 //
-// Two kernels, chosen in gemm_dispatch from the epilogue and K.  The gate + residual epilogue, and a GELU epilogue at
-// K <= 1536, run the persistent ping-pong kernel, which hides the epilogue under the tensor cores.  A bias-only GEMM,
-// and a GELU GEMM at longer K, run gemm_tile_kernel (one CTA per 128 x 192 tile, below), whose K loop is faster.
+// Three kernels, chosen in gemm_route from the epilogue, K and the tile count.  Large-M GEMMs (except the residual
+// epilogue at short K) run gemm_wide_kernel (persistent, 256 x 128 tiles, below), whose K loop moves the fewest bytes
+// per FLOP and whose epilogue runs under the next tile's K loop.  Of the rest, the gate + residual epilogue, and a GELU epilogue at K <= 1536, run the persistent ping-pong kernel, which
+// hides the epilogue under the tensor cores; a bias-only GEMM, and a GELU GEMM at longer K, run gemm_tile_kernel (one
+// CTA per 128 x 192 tile, below), whose K loop is faster.
 //
 // Persistent ping-pong kernel: min(tiles, SMs) CTAs, each walking the 128 x 128 output tiles blockIdx.x, + gridDim.x, ...
 // N-fastest (so the 128-row A panel is reused from L2 across its N tiles), two warpgroups and one warp:
@@ -29,6 +31,7 @@ constexpr int kBM = 128;
 constexpr int kBN = 128;
 constexpr int kBK = 64;
 constexpr int kPersistentGeluMaxK = 1536;  // longest K at which a GELU epilogue runs on the persistent kernel
+constexpr long long kWideMinTiles = 2048;  // fewest 256 x 128 tiles at which gemm_route picks gemm_wide_kernel
 // two consumer warpgroups + one producer warp; ptxas allots 168 registers per thread: 128 accumulators + the epilogue
 constexpr int kGemmThreads = 288;
 
@@ -65,6 +68,84 @@ struct EpiArgs {
   const uint8_t* x_mask;  // [B, T] or null
   int gate_row, B, T, S;
 };
+
+// ---- the epilogue of one consumer's 128 x 128 block (both persistent kernels) ---------------------------------------
+// acc[hm] holds rows 64 hm .. 64 hm + 63 of the block whose first output element is (m0, n0); the 16-bit result goes
+// to the consumer's 128B-swizzled staging tile at my_c ([kBN/64][128 rows][128 B]), for the caller to TMA-store.  ACT 2
+// reads resid from the same slots, where the producer's TMA load lands it (resid_full completes phase `parity`).
+template <int ACT>
+__device__ __forceinline__ void gemm_epilogue(const float (&acc)[2][64], uint32_t my_c, int m0, int n0, int M, int N,
+                                              const bf16* __restrict__ bias, const EpiArgs& ep, uint64_t* resid_full,
+                                              uint32_t parity, int warp, int lane) {
+  // thread rows: rl + 8 h + 64 hm for acc[hm][.. 2 h / 2 h + 1].  Every row of a thread has the same row % 8, so the
+  // 128B swizzle of the staging chunk is one XOR per 8-column group: conflict-free (the 8 rows of a store land in 8
+  // different 16-byte units).
+  const int rl = warp * 16 + (lane >> 2);
+  const uint32_t c_row = my_c + rl * 128 + (lane & 3) * 4;
+  int gate_off[2][2] = {{-1, -1}, {-1, -1}};  // element offset of the row's gate vector in mod, -1: none
+  if (ACT == 2 && ep.gate_row >= 0) {
+#pragma unroll
+    for (int hm = 0; hm < 2; ++hm)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int grow = m0 + rl + 8 * h + 64 * hm;
+        if (grow < M) {
+          const int bt = grow / ep.S;
+          const int bb = bt / ep.T;
+          const int sel = (ep.x_mask != nullptr && ep.x_mask[bt] == 0) ? 1 : 0;
+          gate_off[hm][h] = ((sel * ep.B + bb) * 6 + ep.gate_row) * N;
+        }
+      }
+  }
+  if (ACT == 2) mbar_wait_quiet(resid_full, parity);  // the resid block is in the staging tile
+#pragma unroll
+  for (int jj = 0; jj < kBN / 8; ++jj) {
+    const int col = jj * 8 + 2 * (lane & 3);  // column inside the tile
+    const int gcol = n0 + col;
+    float2 b2 = make_float2(0.f, 0.f);
+    if (bias != nullptr && gcol < N) b2 = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(bias + gcol)));
+#pragma unroll
+    for (int hm = 0; hm < 2; ++hm)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = rl + 8 * h + 64 * hm;
+        float x0 = acc[hm][4 * jj + 2 * h] + b2.x, x1 = acc[hm][4 * jj + 2 * h + 1] + b2.y;
+        const uint32_t dst = c_row + (jj >> 3) * (kBM * 128) + (8 * h + 64 * hm) * 128 + (((jj & 7) ^ (rl & 7)) << 4);
+        if (ACT == 1) {
+          x0 = gelu_tanh_f(rbf(x0));
+          x1 = gelu_tanh_f(rbf(x1));
+        }
+        if (ACT == 2) {
+          if (m0 + row < M && gcol < N) {
+            float y0 = rbf(x0), y1 = rbf(x1);  // the Linear's 16-bit output
+            if (gate_off[hm][h] >= 0) {
+              const float2 g = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(ep.mod + gate_off[hm][h] + gcol)));
+              y0 = rbf(g.x * y0);  // bf16(gate * y)
+              y1 = rbf(g.y * y1);
+            }
+            uint32_t r;
+            asm volatile("ld.shared.b32 %0, [%1];" : "=r"(r) : "r"(dst));  // resid, landed by TMA in the same slot
+            const float2 xr = unpack_bf16x2(r);
+            x0 = xr.x + y0;  // residual add (rounded by the pack below)
+            x1 = xr.y + y1;
+          }
+        }
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(dst), "r"(pack_bf16x2(x0, x1)) : "memory");  // ACT 3: rbf(x)
+      }
+  }
+  if (ACT == 3) {
+    // erf-GELU in a second pass over the thread's own staging slots (as in gemm_tile_kernel)
+#pragma unroll 8
+    for (int i = 0; i < kBN / 2; ++i) {
+      const int jj = i >> 2, hm = (i >> 1) & 1, h = i & 1;
+      const uint32_t dst = c_row + (jj >> 3) * (kBM * 128) + (8 * h + 64 * hm) * 128 + (((jj & 7) ^ (rl & 7)) << 4);
+      uint32_t r;
+      asm volatile("ld.shared.b32 %0, [%1];" : "=r"(r) : "r"(dst));
+      const float2 v = unpack_bf16x2(r);
+      asm volatile("st.shared.b32 [%0], %1;" ::"r"(dst), "r"(pack_bf16x2(gelu_erf_f(v.x), gelu_erf_f(v.y))) : "memory");
+    }
+  }
+}
 
 // ---- one CTA per 128 x BN tile (BN = 192 where it divides N): bias only, or GELU at long K --------------------------
 // Without an epilogue to hide, the persistent kernel's 128 x 128 tile loses to this one: its mainloop moves 32 KB from L2
@@ -339,75 +420,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
     wgmma_wait<0>();
     if (t == 0) mbar_arrive(&empty[(n_base + num_kb - 1) % kStages]);
 
-    // ===================== epilogue =====================
-    // thread rows: rl + 8 h + 64 hm for acc[hm][.. 2 h / 2 h + 1].  Every row of a thread has the same row % 8, so the
-    // 128B swizzle of the staging chunk is one XOR per 8-column group: conflict-free (the 8 rows of a store land in 8
-    // different 16-byte units).
-    const int rl = warp * 16 + (lane >> 2);
-    const uint32_t c_row = my_c + rl * 128 + (lane & 3) * 4;
-    int gate_off[2][2] = {{-1, -1}, {-1, -1}};  // element offset of the row's gate vector in mod, -1: none
-    if (ACT == 2 && ep.gate_row >= 0) {
-#pragma unroll
-      for (int hm = 0; hm < 2; ++hm)
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int grow = m0 + rl + 8 * h + 64 * hm;
-          if (grow < M) {
-            const int bt = grow / ep.S;
-            const int bb = bt / ep.T;
-            const int sel = (ep.x_mask != nullptr && ep.x_mask[bt] == 0) ? 1 : 0;
-            gate_off[hm][h] = ((sel * ep.B + bb) * 6 + ep.gate_row) * N;
-          }
-        }
-    }
-    if (ACT == 2) mbar_wait_quiet(&c_full[c], u & 1);  // the resid block is in the staging tile
-#pragma unroll
-    for (int jj = 0; jj < kBN / 8; ++jj) {
-      const int col = jj * 8 + 2 * (lane & 3);  // column inside the tile
-      const int gcol = n0 + col;
-      float2 b2 = make_float2(0.f, 0.f);
-      if (bias != nullptr && gcol < N) b2 = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(bias + gcol)));
-#pragma unroll
-      for (int hm = 0; hm < 2; ++hm)
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int row = rl + 8 * h + 64 * hm;
-          float x0 = acc[hm][4 * jj + 2 * h] + b2.x, x1 = acc[hm][4 * jj + 2 * h + 1] + b2.y;
-          const uint32_t dst = c_row + (jj >> 3) * (kBM * 128) + (8 * h + 64 * hm) * 128 + (((jj & 7) ^ (rl & 7)) << 4);
-          if (ACT == 1) {
-            x0 = gelu_tanh_f(rbf(x0));
-            x1 = gelu_tanh_f(rbf(x1));
-          }
-          if (ACT == 2) {
-            if (m0 + row < M && gcol < N) {
-              float y0 = rbf(x0), y1 = rbf(x1);  // the Linear's 16-bit output
-              if (gate_off[hm][h] >= 0) {
-                const float2 g = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(ep.mod + gate_off[hm][h] + gcol)));
-                y0 = rbf(g.x * y0);  // bf16(gate * y)
-                y1 = rbf(g.y * y1);
-              }
-              uint32_t r;
-              asm volatile("ld.shared.b32 %0, [%1];" : "=r"(r) : "r"(dst));  // resid, landed by TMA in the same slot
-              const float2 xr = unpack_bf16x2(r);
-              x0 = xr.x + y0;  // residual add (rounded by the pack below)
-              x1 = xr.y + y1;
-            }
-          }
-          asm volatile("st.shared.b32 [%0], %1;" ::"r"(dst), "r"(pack_bf16x2(x0, x1)) : "memory");  // ACT 3: rbf(x)
-        }
-    }
-    if (ACT == 3) {
-      // erf-GELU in a second pass over the thread's own staging slots (as in gemm_tile_kernel)
-#pragma unroll 8
-      for (int i = 0; i < kBN / 2; ++i) {
-        const int jj = i >> 2, hm = (i >> 1) & 1, h = i & 1;
-        const uint32_t dst = c_row + (jj >> 3) * (kBM * 128) + (8 * h + 64 * hm) * 128 + (((jj & 7) ^ (rl & 7)) << 4);
-        uint32_t r;
-        asm volatile("ld.shared.b32 %0, [%1];" : "=r"(r) : "r"(dst));
-        const float2 v = unpack_bf16x2(r);
-        asm volatile("st.shared.b32 [%0], %1;" ::"r"(dst), "r"(pack_bf16x2(gelu_erf_f(v.x), gelu_erf_f(v.y))) : "memory");
-      }
-    }
+    gemm_epilogue<ACT>(acc, my_c, m0, n0, M, N, bias, ep, &c_full[c], u & 1, warp, lane);
     fence_proxy_async_smem();
     named_bar_sync(3 + c, 128);
     if (t == 0) {
@@ -440,6 +453,252 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tw, const CUten
   return check_launch("gemm_wgmma");
 }
 
+// ---- persistent cooperative kernel on 256 x 128 tiles: the large-M Linears --------------------------------------------
+// min(tiles, SMs) CTAs walk the 256 x 128 output tiles with a static stride, N-fastest.  Both consumer warpgroups work on
+// the same tile, warpgroup c on rows 128 c .. 128 c + 127, with the same 2 x wgmma.m64n128k16 per k16 step as a consumer
+// of gemm_wgmma_kernel, and both read one W stage: a stage is A 256x64 + W 128x64 = 48 KB per 4.2 MFLOP, a quarter
+// fewer L2 -> SM bytes per FLOP than the 128 x 128 tile.
+// Without a second tile to ping-pong with, the epilogue is split so that little of it stays off the tensor cores.  Every
+// epilogue starts from y = bf16(acc + bias): the consumers store that into their half of the staging tile (the bias-only
+// epilogue of gemm_epilogue) and go on to the next tile's mainloop; three epilogue warps then apply the rest in place --
+// tanh-GELU(y), erf-GELU(y), or resid + [bf16(gate * y)] with resid read from global memory -- and TMA-store the tile.
+// Every step sees the same 16-bit y and does the same fp32 arithmetic as in gemm_wgmma_kernel, so the outputs are
+// bit-identical.  Barriers per staging half c: st_full[c] (the consumer's 128 threads have written y), st_free[c] (the
+// tile's TMA store has read the half).
+constexpr int kWideThreads = 384;  // two consumer warpgroups, three epilogue warps, one producer warp
+constexpr int kWideEpiThreads = 96;
+
+struct WideCfg {
+  static constexpr int kBMw = 2 * kBM;
+  static constexpr int kABytes = kBMw * kBK * 2;  // two 128-row TMA boxes
+  static constexpr int kStageBytes = kABytes + kBN * kBK * 2;
+  static constexpr int kCBytes = kBM * kBN * 2;  // one consumer's half of the staging tile
+  static constexpr int kStages = 3;
+  // 3 x 48 KB ring + 2 x 32 KB staging, + 1024 for manual alignment, + 256 for barriers: 214 272 B of the 227 KB
+  static constexpr int kSmemBytes = kStages * kStageBytes + 2 * kCBytes + 1024 + 256;
+};
+
+template <int ACT>
+__global__ void __launch_bounds__(kWideThreads, 1)
+gemm_wide_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_w,
+                 const __grid_constant__ CUtensorMap tm_c, const bf16* __restrict__ bias, int M, int N, int K,
+                 const EpiArgs ep) {
+  using Cfg = WideCfg;
+  constexpr int kStages = Cfg::kStages;
+  extern __shared__ unsigned char smem_dyn[];
+  unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~uintptr_t(1023));
+  unsigned char* smem_ab = smem;                              // [kStages][A 32 KB | W 16 KB]
+  unsigned char* smem_c = smem + kStages * Cfg::kStageBytes;  // [consumer][kBN/64][128 rows][128 B] swizzled
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem_c + 2 * Cfg::kCBytes);  // [kStages]
+  uint64_t* empty = full + kStages;                                         // [kStages]
+  uint64_t* st_full = empty + kStages;  // [2]
+  uint64_t* st_free = st_full + 2;      // [2]
+
+  const int wg = threadIdx.x >> 7;
+  const int tiles_n = (N + kBN - 1) / kBN;
+  const int tiles = ((M + Cfg::kBMw - 1) / Cfg::kBMw) * tiles_n;
+  const int num_kb = (K + kBK - 1) / kBK;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tm_a);
+    tma_prefetch_desc(&tm_w);
+    tma_prefetch_desc(&tm_c);
+    for (int i = 0; i < kStages; ++i) {
+      mbar_init(&full[i], 1);
+      mbar_init(&empty[i], 2);  // one arrival per consumer warpgroup
+    }
+    for (int i = 0; i < 2; ++i) {
+      mbar_init(&st_full[i], 128);
+      mbar_init(&st_free[i], 1);
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (wg == 2) {
+    if (threadIdx.x == 256 + kWideEpiThreads) {
+      // ===================== TMA producer (warp 11) =====================
+      int n = 0;  // k-blocks loaded so far: the position in the ring, carried over between tiles
+      for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+        const int m0 = (tile / tiles_n) * Cfg::kBMw, n0 = (tile % tiles_n) * kBN;
+        const bool lower = m0 + kBM < M;  // the lower half has rows inside M (else its A loads are skipped)
+        for (int kb = 0; kb < num_kb; ++kb, ++n) {
+          const int s = n % kStages;
+          mbar_wait_quiet(&empty[s], ((n / kStages) & 1) ^ 1);
+          unsigned char* sa = smem_ab + s * Cfg::kStageBytes;
+          mbar_arrive_expect_tx(&full[s], Cfg::kStageBytes - (lower ? 0 : kBM * kBK * 2));
+          tma_load_2d(&tm_a, &full[s], sa, kb * kBK, m0);
+          if (lower) tma_load_2d(&tm_a, &full[s], sa + kBM * kBK * 2, kb * kBK, m0 + kBM);
+          tma_load_2d(&tm_w, &full[s], sa + Cfg::kABytes, kb * kBK, n0);
+        }
+      }
+    } else if (threadIdx.x < 256 + kWideEpiThreads) {
+      // ===================== epilogue warps 8-10: the staged y -> the output, under the next mainloop ===============
+      const int e = threadIdx.x - 256;
+      const uint32_t c0 = smem_u32(smem_c);
+      int j = 0;
+      for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x, ++j) {
+        const int m0 = (tile / tiles_n) * Cfg::kBMw, n0 = (tile % tiles_n) * kBN;
+        mbar_wait_quiet(&st_full[0], j & 1);
+        mbar_wait_quiet(&st_full[1], j & 1);
+        if (ACT != 0) {
+          // 16-byte unit u of the staging tile = 8 columns of one row: u = ((half * 2 + chunk) * 128 + row) * 8 + slot,
+          // the slot holding column group slot ^ (row & 7) of the 128B swizzle
+#pragma unroll 2
+          for (int u = e; u < 2 * Cfg::kCBytes / 16; u += kWideEpiThreads) {
+            const int row = (u >> 3) & (kBM - 1), hc = u >> 10;
+            const int grow = m0 + (hc >> 1) * kBM + row;
+            const int gcol = n0 + (hc & 1) * 64 + (((u & 7) ^ (row & 7)) << 3);
+            if (ACT == 2 && (grow >= M || gcol >= N)) continue;
+            const uint32_t addr = c0 + u * 16;
+            uint32_t v[4];
+            asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]) : "r"(addr));
+            if (ACT == 2) {
+              const uint4 r4 = *reinterpret_cast<const uint4*>(ep.resid + (size_t)grow * N + gcol);  // may alias the output
+              const uint32_t r[4] = {r4.x, r4.y, r4.z, r4.w};
+              uint32_t g[4] = {0, 0, 0, 0};
+              if (ep.gate_row >= 0) {
+                const int bt = grow / ep.S;
+                const int bb = bt / ep.T;
+                const int sel = (ep.x_mask != nullptr && ep.x_mask[bt] == 0) ? 1 : 0;
+                const uint4 g4 = __ldg(reinterpret_cast<const uint4*>(ep.mod + ((sel * ep.B + bb) * 6 + ep.gate_row) * N + gcol));
+                g[0] = g4.x, g[1] = g4.y, g[2] = g4.z, g[3] = g4.w;
+              }
+#pragma unroll
+              for (int i = 0; i < 4; ++i) {
+                float2 y = unpack_bf16x2(v[i]);  // the Linear's 16-bit output
+                if (ep.gate_row >= 0) {
+                  const float2 gg = unpack_bf16x2(g[i]);
+                  y.x = rbf(gg.x * y.x);  // bf16(gate * y)
+                  y.y = rbf(gg.y * y.y);
+                }
+                const float2 xr = unpack_bf16x2(r[i]);
+                v[i] = pack_bf16x2(xr.x + y.x, xr.y + y.y);  // residual add, rounded by the pack
+              }
+            } else {
+#pragma unroll
+              for (int i = 0; i < 4; ++i) {
+                const float2 y = unpack_bf16x2(v[i]);
+                v[i] = ACT == 1 ? pack_bf16x2(gelu_tanh_f(y.x), gelu_tanh_f(y.y)) : pack_bf16x2(gelu_erf_f(y.x), gelu_erf_f(y.y));
+              }
+            }
+            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3])
+                         : "memory");
+          }
+          fence_proxy_async_smem();
+        }
+        named_bar_sync(1, kWideEpiThreads);
+        if (e == 0) {
+#pragma unroll 1
+          for (int h = 0; h < 2; ++h)
+            for (int ch = 0; ch < kBN / 64; ++ch)
+              if (m0 + h * kBM < M && n0 + ch * 64 < N)
+                tma_store_2d_s(&tm_c, c0 + h * Cfg::kCBytes + ch * (kBM * 128), n0 + ch * 64, m0 + h * kBM);
+          tma_store_commit();
+          tma_store_wait_read0();  // the consumers write the next tile's y into the halves after this
+          mbar_arrive(&st_free[0]);
+          mbar_arrive(&st_free[1]);
+        }
+      }
+      if (e == 0) tma_store_wait0();
+    }
+    return;
+  }
+
+  // ===================== consumers: warpgroup c takes rows 128 c .. 128 c + 127 of every tile of the CTA ==============
+  const int c = wg;
+  const int t = threadIdx.x & 127;
+  const int warp = t >> 5, lane = t & 31;
+  const uint32_t my_c = smem_u32(smem_c) + c * Cfg::kCBytes;
+  const uint32_t ab0 = smem_u32(smem_ab);
+  int j = 0;
+  for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x, ++j) {
+    const int m0 = (tile / tiles_n) * Cfg::kBMw + c * kBM, n0 = (tile % tiles_n) * kBN;
+    float acc[2][64];
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int i = 0; i < 64; ++i) acc[h][i] = 0.f;
+
+    const int n_base = j * num_kb;  // ring position of this tile's first k-block
+    for (int kb = 0; kb < num_kb; ++kb) {
+      const int n = n_base + kb, s = n % kStages;
+      mbar_wait_quiet(&full[s], (n / kStages) & 1);
+      const uint32_t sa = ab0 + s * Cfg::kStageBytes + c * (kBM * kBK * 2);
+      const uint32_t sw = ab0 + s * Cfg::kStageBytes + Cfg::kABytes;
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kBK / 16; ++k) {
+        const uint64_t dw = wgmma_desc_sw128(sw + 32 * k);
+        wgmma_m64n128k16_ss(acc[0], wgmma_desc_sw128(sa + 32 * k), dw, 1u);
+        wgmma_m64n128k16_ss(acc[1], wgmma_desc_sw128(sa + 64 * 128 + 32 * k), dw, 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();  // the group of k-block kb - 1 has retired: its stage can be refilled
+      if (kb > 0 && t == 0) mbar_arrive(&empty[(n - 1) % kStages]);
+    }
+    wgmma_wait<0>();
+    if (t == 0) mbar_arrive(&empty[(n_base + num_kb - 1) % kStages]);
+
+    if (j > 0) mbar_wait_quiet(&st_free[c], (j - 1) & 1);  // the previous tile's store has read this half
+    gemm_epilogue<0>(acc, my_c, m0, n0, M, N, bias, ep, nullptr, 0, warp, lane);  // y = bf16(acc + bias)
+    fence_proxy_async_smem();  // bias only: the TMA store reads y as written
+    mbar_arrive(&st_full[c]);
+  }
+}
+
+template <int ACT>
+static int launch_gemm_wide(const CUtensorMap& ta, const CUtensorMap& tw, const CUtensorMap& tc, const bf16* bias, int M,
+                            int N, int K, cudaStream_t st, const EpiArgs& ep) {
+  static bool attr = false;
+  if (!attr) {
+    cudaError_t e = cudaFuncSetAttribute(gemm_wide_kernel<ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         WideCfg::kSmemBytes);
+    if (e != cudaSuccess) return fail(VSB_ERR_CUDA, "gemm: smem attr: %s", cudaGetErrorString(e));
+    attr = true;
+  }
+  const long long tiles = (long long)((M + WideCfg::kBMw - 1) / WideCfg::kBMw) * ((N + kBN - 1) / kBN);
+  const int grid = tiles < num_sms() ? int(tiles) : num_sms();
+  gemm_wide_kernel<ACT><<<grid, kWideThreads, WideCfg::kSmemBytes, st>>>(ta, tw, tc, bias, M, N, K, ep);
+  return check_launch("gemm_wide");
+}
+
+enum class GemmKernel { kTile128, kTile192, kPingPong, kWide };
+
+// Which kernel runs a GEMM; act: 0 none, 1 tanh-GELU, 2 fused residual, 3 erf-GELU.
+static GemmKernel gemm_route(int M, int N, int K, int act) {
+  // The 256 x 128 kernel against the kernel each shape ran on before (bench_gemm.py, H100 80GB HBM3, 700 W, SM clock
+  // 1980 MHz, bit-identical outputs; DESIGN.md section 9):
+  //   bias only (was gemm_tile_kernel<192>): K 1152 1.24x (N 3456) / 1.15x (N 1152), K 1920 1.12x, K 2304 1.07x,
+  //     K 4608 1.05x
+  //   tanh-GELU: K 1152 1.20x, K 1536 1.20x (both were persistent), K 1920 1.16x, K 2304 1.16x, K 3072 1.12x
+  //   erf-GELU, K 2304: 1.09x;  gate + residual (was persistent): K 1152 0.55x, K 4608 1.24x
+  // The residual epilogue reads resid from global memory in the epilogue warps, which a K loop of 1152 does not hide.
+  // It runs at 2048 tiles or more: the fewest it was measured at (CogVideoX-2B, 2085).
+  const long long wide_tiles = (long long)((M + WideCfg::kBMw - 1) / WideCfg::kBMw) * ((N + kBN - 1) / kBN);
+  if (wide_tiles >= kWideMinTiles && (act != 2 || K >= 4608))
+    return GemmKernel::kWide;
+  // The persistent kernel's K loop is slower than the one-tile-per-CTA kernel's (0.671 against 0.521 ms per 1152 of K at
+  // N 1152, H100 SXM, DESIGN.md section 9); what it saves per tile is the fill, the store and the epilogue.  The gate +
+  // residual epilogue saves more than the K loop costs at every K measured (up to 4608); a bias-only epilogue never does;
+  // a GELU epilogue only while K is short.
+  if (act == 0 || ((act == 1 || act == 3) && K > kPersistentGeluMaxK)) {
+    // tile width: 192 divides every STDiT3 / CogVideoX / Latte width (1152, 1920, 2304, 3072, 3456, 4608, 7680); narrow
+    // outputs and widths that 128 divides but 192 does not take 128
+    return (N % 192 == 0 || (N > 192 && N % 128 != 0)) ? GemmKernel::kTile192 : GemmKernel::kTile128;
+  }
+  return GemmKernel::kPingPong;
+}
+
+static const char* gemm_kernel_name(GemmKernel k, int act) {
+  static const char* const names[4][4] = {
+      {"gemm_tile_kernel<128, 0>", "gemm_tile_kernel<128, 1>", "", "gemm_tile_kernel<128, 3>"},
+      {"gemm_tile_kernel<192, 0>", "gemm_tile_kernel<192, 1>", "", "gemm_tile_kernel<192, 3>"},
+      {"", "gemm_wgmma_kernel<1>", "gemm_wgmma_kernel<2>", "gemm_wgmma_kernel<3>"},
+      {"gemm_wide_kernel<0>", "gemm_wide_kernel<1>", "gemm_wide_kernel<2>", "gemm_wide_kernel<3>"}};
+  return names[int(k)][act];
+}
+
 // act: 0 none, 1 tanh-GELU, 2 fused residual (ep->resid != nullptr), 3 erf-GELU
 static int gemm_dispatch(const void* A, const void* W, const void* bias, void* out, int M, int N, int K, int act,
                          cudaStream_t st, const EpiArgs& ep) {
@@ -452,17 +711,11 @@ static int gemm_dispatch(const void* A, const void* W, const void* bias, void* o
   int rc = make_tmap_bf16(&ta, A, 2, da, sa, ba, CU_TENSOR_MAP_SWIZZLE_128B);
   if (rc) return rc;
   const bf16* b = (const bf16*)bias;
-  // The persistent kernel's K loop is slower than the one-tile-per-CTA kernel's (0.671 against 0.521 ms per 1152 of K at
-  // N 1152, H100 SXM, DESIGN.md section 9); what it saves per tile is the fill, the store and the epilogue.  The gate +
-  // residual epilogue saves more than the K loop costs at every K measured (up to 4608); a bias-only epilogue never does;
-  // a GELU epilogue only while K is short.
-  if (act == 0 || ((act == 1 || act == 3) && K > kPersistentGeluMaxK)) {
-    // tile width: 192 divides every STDiT3 / CogVideoX / Latte width (1152, 1920, 2304, 3072, 3456, 4608, 7680); narrow
-    // outputs and widths that 128 divides but 192 does not take 128
-    const bool wide = N % 192 == 0 || (N > 192 && N % 128 != 0);
+  const GemmKernel kern = gemm_route(M, N, K, act);
+  if (kern == GemmKernel::kTile128 || kern == GemmKernel::kTile192) {
 #define VSB_TILE_CASE(a)                                                                                      \
-  if (act == a) return wide ? launch_gemm_tile<192, a>(A, W, b, out, M, N, K, ta, st)                         \
-                            : launch_gemm_tile<128, a>(A, W, b, out, M, N, K, ta, st);
+  if (act == a) return kern == GemmKernel::kTile192 ? launch_gemm_tile<192, a>(A, W, b, out, M, N, K, ta, st) \
+                                                    : launch_gemm_tile<128, a>(A, W, b, out, M, N, K, ta, st);
     VSB_TILE_CASE(0)
     VSB_TILE_CASE(1)
     VSB_TILE_CASE(3)
@@ -482,6 +735,12 @@ static int gemm_dispatch(const void* A, const void* W, const void* bias, void* o
     if (rc) return rc;
   } else {
     tr = tc;  // unused
+  }
+  if (kern == GemmKernel::kWide) {
+    if (act == 0) return launch_gemm_wide<0>(ta, tw, tc, b, M, N, K, st, ep);
+    if (act == 1) return launch_gemm_wide<1>(ta, tw, tc, b, M, N, K, st, ep);
+    if (act == 2) return launch_gemm_wide<2>(ta, tw, tc, b, M, N, K, st, ep);
+    return launch_gemm_wide<3>(ta, tw, tc, b, M, N, K, st, ep);
   }
   if (act == 3) return launch_gemm<3>(ta, tw, tc, tr, b, M, N, K, st, ep);
   if (act == 2) return launch_gemm<2>(ta, tw, tc, tr, b, M, N, K, st, ep);
@@ -516,3 +775,12 @@ extern "C" int VSB_API(vsb_gemm_bias_residual)(const vsb_bf16* A, const vsb_bf16
   EpiArgs ep{(const bf16*)resid, (const bf16*)mod, x_mask, gate_row, B, T, S};
   return gemm_dispatch(A, W, bias, out, M, N, K, 2, (cudaStream_t)stream, ep);
 }
+
+#ifndef VSB_HALF
+// The kernel gemm_dispatch picks for a shape (the same for both 16-bit types), see include/vsb200.h.
+extern "C" const char* vsb_gemm_kernel_name(int M, int N, int K, int act, int residual) {
+  if (M <= 0 || N <= 0 || K <= 0 || act < 0 || act > 2 || (residual && act != 0)) return "";
+  const int epi = residual ? 2 : (act == 2 ? 3 : act);
+  return gemm_kernel_name(gemm_route(M, N, K, epi), epi);
+}
+#endif

@@ -556,6 +556,15 @@ def gemm_bias_residual(a, w, bias, resid, mod=None, x_mask_u8=None, gate_row: in
     return out
 
 
+def gemm_kernel_name(M: int, N: int, K: int, act: int = 0, residual: bool = False) -> str:
+    """The kernel instance gemm_bias_act (act) or gemm_bias_residual (residual=True) launches for an M x N x K GEMM."""
+    lib = _lib.load()
+    name = lib.vsb_gemm_kernel_name(M, N, K, act, int(residual)).decode()
+    if not name:
+        raise _lib.VsbError(f"gemm_kernel_name: bad arguments M={M} N={N} K={K} act={act} residual={residual}")
+    return name
+
+
 def attn_flash(q, k, v, nb, nq, nk, H, D, q_row_stride, q_batch_stride, kv_row_stride, kv_batch_stride, scale,
                kv_lens: Optional[Sequence[int]] = None, out=None, out_row_stride=None, out_batch_stride=None):
     """q/k/v: tensors whose data_ptr() is the first element of the strided view (may be slices of one buffer).
