@@ -15,6 +15,10 @@
   gelu_k1536   tanh-GELU at K 1536 and 3072 (M 36 000, N 4608): with fc1 (K 1152) and the two above, where the GELU
   gelu_k3072   epilogue stops paying for a kernel of its own
   t_block      the t_block Linear: M = 2 (a CFG pair), N 6912, K 1152
+  m4096_*      M 4096 and N 4608 (m4096_*) or N 1024 (n1024_*): too few tiles for the 256 x 128 kernel, so these time
+  n1024_*      the instances no shape above reaches: the ping-pong kernel's tanh- / erf-GELU epilogues (K 1152), the
+               one-tile-per-CTA kernel's GELU epilogues (K 2304) at tile widths 192 and 128, and its 128-wide bias-only
+               tile (n1024, K 1152)
 
     python bench_gemm.py [--iters 20] [--warmup 3] [--rounds 3] [--shapes a,b] [--no-cublas] [--out FILE.json]
 
@@ -57,6 +61,13 @@ SHAPES = {
     "gelu_k1536": (36000, 4608, 1536, torch.bfloat16, 1),
     "gelu_k3072": (36000, 4608, 3072, torch.bfloat16, 1),
     "t_block": (2, 6912, 1152, torch.bfloat16, 0),
+    "m4096_tanh": (4096, 4608, 1152, torch.bfloat16, 1),
+    "m4096_erf": (4096, 4608, 1152, torch.bfloat16, 2),
+    "m4096_tanh_k2304": (4096, 4608, 2304, torch.bfloat16, 1),
+    "m4096_erf_k2304": (4096, 4608, 2304, torch.bfloat16, 2),
+    "n1024": (4096, 1024, 1152, torch.bfloat16, 0),
+    "n1024_tanh": (4096, 1024, 2304, torch.bfloat16, 1),
+    "n1024_erf": (4096, 1024, 2304, torch.bfloat16, 2),
 }
 B720, T720, S720 = 2, 20, 3600
 

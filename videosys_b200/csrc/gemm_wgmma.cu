@@ -30,13 +30,17 @@ namespace vsb {
 constexpr int kBM = 128;
 constexpr int kBN = 128;
 constexpr int kBK = 64;
+constexpr int kABox = kBM * kBK * 2;       // one 128-row A box of a k-block
 constexpr int kPersistentGeluMaxK = 1536;  // longest K at which a GELU epilogue runs on the persistent kernel
 constexpr long long kWideMinTiles = 2048;  // fewest 256 x 128 tiles at which gemm_route picks gemm_wide_kernel
-// two consumer warpgroups + one producer warp; ptxas allots 168 registers per thread: 128 accumulators + the epilogue
-constexpr int kGemmThreads = 288;
 
-struct GemmCfg {
-  static constexpr int kABytes = kBM * kBK * 2;
+// Each kernel's tile, launch and shared memory.  kStageBytes: the A boxes then the W box of one k-block.
+struct GemmCfg {  // gemm_wgmma_kernel
+  static constexpr int kTileM = kBM, kTileN = kBN;
+  static constexpr bool kPersistent = true;
+  // two consumer warpgroups + one producer warp; ptxas allots 168 registers per thread: 128 accumulators + the epilogue
+  static constexpr int kThreads = 288;
+  static constexpr int kABytes = kABox;
   static constexpr int kStageBytes = (kBM + kBN) * kBK * 2;
   static constexpr int kCBytes = kBM * kBN * 2;  // one staging tile: [kBN/64][128 rows][128 B] swizzled
   static constexpr int kStages = 5;
@@ -44,6 +48,33 @@ struct GemmCfg {
   static constexpr int kSmemBytes = kStages * kStageBytes + 2 * kCBytes + 1024 + 256;
 };
 
+template <int BN>
+struct TileCfg {  // gemm_tile_kernel<BN, .>
+  static constexpr int kTileM = kBM, kTileN = BN;
+  static constexpr bool kPersistent = false;
+  static constexpr int kThreads = 384;
+  static constexpr int kABytes = kABox;
+  static constexpr int kStageBytes = (kBM + BN) * kBK * 2;
+  static constexpr int kCBytes = kBM * BN * 2;
+  static constexpr int kStages = 4;
+  // + 1024 for manual alignment, + 256 for barriers
+  static constexpr int kSmemBytes = kStages * kStageBytes + kCBytes + 1024 + 256;
+};
+
+constexpr int kWideEpiThreads = 96;
+struct WideCfg {  // gemm_wide_kernel
+  static constexpr int kTileM = 2 * kBM, kTileN = kBN;
+  static constexpr bool kPersistent = true;
+  static constexpr int kThreads = 384;  // two consumer warpgroups, three epilogue warps, one producer warp
+  static constexpr int kABytes = 2 * kABox;  // two 128-row TMA boxes
+  static constexpr int kStageBytes = kABytes + kBN * kBK * 2;
+  static constexpr int kCBytes = kBM * kBN * 2;  // one consumer's half of the staging tile
+  static constexpr int kStages = 3;
+  // 3 x 48 KB ring + 2 x 32 KB staging, + 1024 for manual alignment, + 256 for barriers: 214 272 B of the 227 KB
+  static constexpr int kSmemBytes = kStages * kStageBytes + 2 * kCBytes + 1024 + 256;
+};
+
+// ---- the epilogue's element functions: every kernel applies them to y = bf16(acc + bias), two adjacent columns -------
 __device__ __forceinline__ float gelu_tanh_f(float x) {
   // torch GELU(approximate='tanh') = 0.5 x (1 + tanh(u)), u = sqrt(2/pi) (x + 0.044715 x^3), rewritten as
   //   x * sigmoid(2u) = x / (1 + 2^(-2 u log2 e)):
@@ -60,6 +91,12 @@ __device__ __forceinline__ float gelu_tanh_f(float x) {
 // exact GELU (F.gelu, approximate='none') as torch's CUDA kernel evaluates it: x * 0.5 * (1 + erf(x / sqrt(2))) in fp32
 __device__ __forceinline__ float gelu_erf_f(float x) { return x * 0.5f * (1.f + erff(x * 0.70710678118654752440f)); }
 
+// ACT 1: tanh-GELU(y), ACT 3: erf-GELU(y)
+template <int ACT>
+__device__ __forceinline__ float2 gelu2(float2 y) {
+  return ACT == 1 ? make_float2(gelu_tanh_f(y.x), gelu_tanh_f(y.y)) : make_float2(gelu_erf_f(y.x), gelu_erf_f(y.y));
+}
+
 // ACT == 2: out = resid + g, g = bf16(gate * y) (gate_row >= 0, per-frame t/t0 select) or g = y (plain residual add),
 // y = bf16(acc + bias): the eager chain of open_sora_transformer_3d.py (Linear, gate multiply, residual add) in the epilogue.
 struct EpiArgs {
@@ -69,100 +106,102 @@ struct EpiArgs {
   int gate_row, B, T, S;
 };
 
-// ---- the epilogue of one consumer's 128 x 128 block (both persistent kernels) ---------------------------------------
+// element offset in mod of output row `row`'s gate vector: row gate_row of its sample's t (or, where x_mask marks the
+// row's frame 0, t0) modulation
+__device__ __forceinline__ int gate_offset(const EpiArgs& ep, int row, int N) {
+  const int bt = row / ep.S;
+  const int bb = bt / ep.T;
+  const int sel = (ep.x_mask != nullptr && ep.x_mask[bt] == 0) ? 1 : 0;
+  return ((sel * ep.B + bb) * 6 + ep.gate_row) * N;
+}
+
+// resid + [bf16(gate * y)], resid and gate packed; the caller's pack rounds the residual add
+__device__ __forceinline__ float2 residual_add2(float2 y, uint32_t resid, bool gated, uint32_t gate) {
+  if (gated) {
+    const float2 g = unpack_bf16x2(gate);
+    y.x = rbf(g.x * y.x);  // bf16(gate * y)
+    y.y = rbf(g.y * y.y);
+  }
+  const float2 r = unpack_bf16x2(resid);
+  return make_float2(r.x + y.x, r.y + y.y);
+}
+
+// ---- one consumer's epilogue: HALVES 64-row halves x BN columns ----------------------------------------------------
 // acc[hm] holds rows 64 hm .. 64 hm + 63 of the block whose first output element is (m0, n0); the 16-bit result goes
-// to the consumer's 128B-swizzled staging tile at my_c ([kBN/64][128 rows][128 B]), for the caller to TMA-store.  ACT 2
+// to the consumer's 128B-swizzled staging rows at my_c ([BN/64][128 rows][128 B]), for the caller to TMA-store.  ACT 2
 // reads resid from the same slots, where the producer's TMA load lands it (resid_full completes phase `parity`).
-template <int ACT>
-__device__ __forceinline__ void gemm_epilogue(const float (&acc)[2][64], uint32_t my_c, int m0, int n0, int M, int N,
-                                              const bf16* __restrict__ bias, const EpiArgs& ep, uint64_t* resid_full,
-                                              uint32_t parity, int warp, int lane) {
+template <int BN, int HALVES, int ACT>
+__device__ __forceinline__ void gemm_epilogue(const float (&acc)[HALVES][BN / 2], uint32_t my_c, int m0, int n0, int M,
+                                              int N, const bf16* __restrict__ bias, const EpiArgs& ep,
+                                              uint64_t* resid_full, uint32_t parity, int warp, int lane) {
   // thread rows: rl + 8 h + 64 hm for acc[hm][.. 2 h / 2 h + 1].  Every row of a thread has the same row % 8, so the
   // 128B swizzle of the staging chunk is one XOR per 8-column group: conflict-free (the 8 rows of a store land in 8
   // different 16-byte units).
   const int rl = warp * 16 + (lane >> 2);
   const uint32_t c_row = my_c + rl * 128 + (lane & 3) * 4;
-  int gate_off[2][2] = {{-1, -1}, {-1, -1}};  // element offset of the row's gate vector in mod, -1: none
-  if (ACT == 2 && ep.gate_row >= 0) {
+  int gate_off[HALVES][2];  // element offset of the row's gate vector in mod, -1: none
 #pragma unroll
-    for (int hm = 0; hm < 2; ++hm)
+  for (int hm = 0; hm < HALVES; ++hm)
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int grow = m0 + rl + 8 * h + 64 * hm;
-        if (grow < M) {
-          const int bt = grow / ep.S;
-          const int bb = bt / ep.T;
-          const int sel = (ep.x_mask != nullptr && ep.x_mask[bt] == 0) ? 1 : 0;
-          gate_off[hm][h] = ((sel * ep.B + bb) * 6 + ep.gate_row) * N;
-        }
-      }
-  }
+    for (int h = 0; h < 2; ++h) {
+      const int grow = m0 + rl + 8 * h + 64 * hm;
+      gate_off[hm][h] = -1;
+      if (ACT == 2 && ep.gate_row >= 0 && grow < M) gate_off[hm][h] = gate_offset(ep, grow, N);
+    }
   if (ACT == 2) mbar_wait_quiet(resid_full, parity);  // the resid block is in the staging tile
 #pragma unroll
-  for (int jj = 0; jj < kBN / 8; ++jj) {
+  for (int jj = 0; jj < BN / 8; ++jj) {
     const int col = jj * 8 + 2 * (lane & 3);  // column inside the tile
     const int gcol = n0 + col;
     float2 b2 = make_float2(0.f, 0.f);
     if (bias != nullptr && gcol < N) b2 = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(bias + gcol)));
 #pragma unroll
-    for (int hm = 0; hm < 2; ++hm)
+    for (int hm = 0; hm < HALVES; ++hm)
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int row = rl + 8 * h + 64 * hm;
-        float x0 = acc[hm][4 * jj + 2 * h] + b2.x, x1 = acc[hm][4 * jj + 2 * h + 1] + b2.y;
         const uint32_t dst = c_row + (jj >> 3) * (kBM * 128) + (8 * h + 64 * hm) * 128 + (((jj & 7) ^ (rl & 7)) << 4);
-        if (ACT == 1) {
-          x0 = gelu_tanh_f(rbf(x0));
-          x1 = gelu_tanh_f(rbf(x1));
+        float2 x = make_float2(acc[hm][4 * jj + 2 * h] + b2.x, acc[hm][4 * jj + 2 * h + 1] + b2.y);
+        if (ACT == 1) x = gelu2<1>(make_float2(rbf(x.x), rbf(x.y)));
+        if (ACT == 2 && m0 + row < M && gcol < N) {
+          const bool gated = gate_off[hm][h] >= 0;
+          const uint32_t g = gated ? __ldg(reinterpret_cast<const uint32_t*>(ep.mod + gate_off[hm][h] + gcol)) : 0u;
+          uint32_t r;
+          asm volatile("ld.shared.b32 %0, [%1];" : "=r"(r) : "r"(dst));  // resid, landed by TMA in the same slot
+          x = residual_add2(make_float2(rbf(x.x), rbf(x.y)), r, gated, g);
         }
-        if (ACT == 2) {
-          if (m0 + row < M && gcol < N) {
-            float y0 = rbf(x0), y1 = rbf(x1);  // the Linear's 16-bit output
-            if (gate_off[hm][h] >= 0) {
-              const float2 g = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(ep.mod + gate_off[hm][h] + gcol)));
-              y0 = rbf(g.x * y0);  // bf16(gate * y)
-              y1 = rbf(g.y * y1);
-            }
-            uint32_t r;
-            asm volatile("ld.shared.b32 %0, [%1];" : "=r"(r) : "r"(dst));  // resid, landed by TMA in the same slot
-            const float2 xr = unpack_bf16x2(r);
-            x0 = xr.x + y0;  // residual add (rounded by the pack below)
-            x1 = xr.y + y1;
-          }
-        }
-        asm volatile("st.shared.b32 [%0], %1;" ::"r"(dst), "r"(pack_bf16x2(x0, x1)) : "memory");  // ACT 3: rbf(x)
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(dst), "r"(pack_bf16x2(x.x, x.y)) : "memory");  // ACT 3: y, see below
       }
   }
   if (ACT == 3) {
-    // erf-GELU in a second pass over the thread's own staging slots (as in gemm_tile_kernel)
+    // erf-GELU in a second pass over the thread's own staging slots, once the accumulators are dead: erff next to the
+    // live accumulators would not fit in the register budget.
 #pragma unroll 8
-    for (int i = 0; i < kBN / 2; ++i) {
-      const int jj = i >> 2, hm = (i >> 1) & 1, h = i & 1;
+    for (int i = 0; i < BN / 8 * HALVES * 2; ++i) {
+      const int jj = i / (2 * HALVES), hm = (i >> 1) % HALVES, h = i & 1;
       const uint32_t dst = c_row + (jj >> 3) * (kBM * 128) + (8 * h + 64 * hm) * 128 + (((jj & 7) ^ (rl & 7)) << 4);
       uint32_t r;
       asm volatile("ld.shared.b32 %0, [%1];" : "=r"(r) : "r"(dst));
-      const float2 v = unpack_bf16x2(r);
-      asm volatile("st.shared.b32 [%0], %1;" ::"r"(dst), "r"(pack_bf16x2(gelu_erf_f(v.x), gelu_erf_f(v.y))) : "memory");
+      const float2 v = gelu2<3>(unpack_bf16x2(r));
+      asm volatile("st.shared.b32 [%0], %1;" ::"r"(dst), "r"(pack_bf16x2(v.x, v.y)) : "memory");
     }
   }
 }
 
-// ---- one CTA per 128 x BN tile (BN = 192 where it divides N): bias only, or GELU at long K --------------------------
-// Without an epilogue to hide, the persistent kernel's 128 x 128 tile loses to this one: its mainloop moves 32 KB from L2
-// per 2.1 MFLOP against 40 KB per 3.1 MFLOP here, and at ~8.7 TB/s both are bound by the L2 -> SM bandwidth, so the wider
-// tile runs the K loop ~20 % faster (DESIGN.md section 9).  Warpgroup 0 is the TMA producer (one thread), warpgroups 1-2
-// own rows 0..63 / 64..127 of the tile; the epilogue adds the bias, [rounds and applies tanh- or erf-GELU,] and
-// TMA-stores the 16-bit tile.
-template <int BN>
-struct TileCfg {
-  static constexpr int kABytes = kBM * kBK * 2;
-  static constexpr int kStageBytes = (kBM + BN) * kBK * 2;
-  static constexpr int kCBytes = kBM * BN * 2;
-  static constexpr int kStages = 4;
-  // + 1024 for manual alignment, + 256 for barriers
-  static constexpr int kSmemBytes = kStages * kStageBytes + kCBytes + 1024 + 256;
-};
-constexpr int kTileThreads = 384;
+// ---- the producer's k-block and the consumers' K loop, shared by the three kernels -----------------------------------
+// Loads k-block kb of the tile at (m0, n0) into ring position n once the consumers have released the slot: a_boxes
+// 128-row A boxes (1 or 2) and the W box.
+template <class Cfg>
+__device__ __forceinline__ void load_k_block(const CUtensorMap* tm_a, const CUtensorMap* tm_w, unsigned char* smem_ab,
+                                             uint64_t* full, uint64_t* empty, int n, int kb, int m0, int n0, int a_boxes) {
+  const int s = n % Cfg::kStages;
+  mbar_wait_quiet(&empty[s], ((n / Cfg::kStages) & 1) ^ 1);
+  unsigned char* sa = smem_ab + s * Cfg::kStageBytes;
+  mbar_arrive_expect_tx(&full[s], a_boxes * kABox + Cfg::kStageBytes - Cfg::kABytes);
+  tma_load_2d(tm_a, &full[s], sa, kb * kBK, m0);
+  if (a_boxes == 2) tma_load_2d(tm_a, &full[s], sa + kABox, kb * kBK, m0 + kBM);
+  tma_load_2d(tm_w, &full[s], sa + Cfg::kABytes, kb * kBK, n0);
+}
 
 template <int BN>
 __device__ __forceinline__ void wgmma_tile(float (&d)[BN / 2], uint64_t da, uint64_t db, uint32_t scale_d) {
@@ -172,10 +211,52 @@ __device__ __forceinline__ void wgmma_tile(float (&d)[BN / 2], uint64_t da, uint
     wgmma_m64n128k16_ss(d, da, db, scale_d);
 }
 
+// One consumer's K loop over the k-blocks at ring positions n_base .. n_base + num_kb - 1: per k16 step one
+// wgmma.m64n{BN}k16 per 64-row half, A from a_off inside the stage.  Each stage is released once the wgmma that read
+// it has retired, all but the last: the caller releases that after its wgmma_wait<0>.
+template <class Cfg, int HALVES>
+__device__ __forceinline__ void consumer_k_loop(float (&acc)[HALVES][Cfg::kTileN / 2], uint32_t ab0, uint32_t a_off,
+                                                uint64_t* full, uint64_t* empty, int n_base, int num_kb, int t) {
+#pragma unroll
+  for (int hm = 0; hm < HALVES; ++hm)
+#pragma unroll
+    for (int i = 0; i < Cfg::kTileN / 2; ++i) acc[hm][i] = 0.f;
+  for (int kb = 0; kb < num_kb; ++kb) {
+    const int n = n_base + kb, s = n % Cfg::kStages;
+    mbar_wait_quiet(&full[s], (n / Cfg::kStages) & 1);
+    const uint32_t sa = ab0 + s * Cfg::kStageBytes + a_off;
+    const uint32_t sw = ab0 + s * Cfg::kStageBytes + Cfg::kABytes;
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < kBK / 16; ++k) {
+      const uint64_t dw = wgmma_desc_sw128(sw + 32 * k);
+#pragma unroll
+      for (int hm = 0; hm < HALVES; ++hm) wgmma_tile<Cfg::kTileN>(acc[hm], wgmma_desc_sw128(sa + hm * (64 * 128) + 32 * k), dw, 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<1>();  // the group of k-block kb - 1 has retired: its stage can be refilled
+    if (kb > 0 && t == 0) mbar_arrive(&empty[(n - 1) % Cfg::kStages]);
+  }
+}
+
+// TMA store from a 32-bit shared-memory address (the consumers keep no 64-bit pointer live across the mainloop)
+__device__ __forceinline__ void tma_store_2d_s(const CUtensorMap* m, uint32_t src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(reinterpret_cast<uint64_t>(m)),
+               "r"(src), "r"(c0), "r"(c1)
+               : "memory");
+}
+
+// ---- one CTA per 128 x BN tile (BN = 192 where it divides N): bias only, or GELU at long K --------------------------
+// Without an epilogue to hide, the persistent kernel's 128 x 128 tile loses to this one: its mainloop moves 32 KB from L2
+// per 2.1 MFLOP against 40 KB per 3.1 MFLOP here, and at ~8.7 TB/s both are bound by the L2 -> SM bandwidth, so the wider
+// tile runs the K loop ~20 % faster (DESIGN.md section 9).  Warpgroup 0 is the TMA producer (one thread), warpgroups 1-2
+// own rows 0..63 / 64..127 of the tile; the epilogue adds the bias, [rounds and applies tanh- or erf-GELU,] and
+// TMA-stores the 16-bit tile.
 template <int BN, int ACT>
-__global__ void __launch_bounds__(kTileThreads, 1)
+__global__ void __launch_bounds__(TileCfg<BN>::kThreads, 1)
 gemm_tile_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_w,
-                 const __grid_constant__ CUtensorMap tm_c, const bf16* __restrict__ bias, int M, int N, int K) {
+                 const __grid_constant__ CUtensorMap tm_c, const __grid_constant__ CUtensorMap tm_r,
+                 const bf16* __restrict__ bias, int M, int N, int K, const EpiArgs ep) {
   using Cfg = TileCfg<BN>;
   constexpr int kStages = Cfg::kStages;
   extern __shared__ unsigned char smem_dyn[];
@@ -203,73 +284,19 @@ gemm_tile_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant
   __syncthreads();
 
   if (wg == 0) {
-    if (threadIdx.x == 0) {
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb % kStages;
-        mbar_wait_quiet(&empty[s], ((kb / kStages) & 1) ^ 1);
-        unsigned char* sa = smem_ab + s * Cfg::kStageBytes;
-        mbar_arrive_expect_tx(&full[s], Cfg::kStageBytes);
-        tma_load_2d(&tm_a, &full[s], sa, kb * kBK, m0);
-        tma_load_2d(&tm_w, &full[s], sa + Cfg::kABytes, kb * kBK, n0);
-      }
-    }
+    if (threadIdx.x == 0)
+      for (int kb = 0; kb < num_kb; ++kb) load_k_block<Cfg>(&tm_a, &tm_w, smem_ab, full, empty, kb, kb, m0, n0, 1);
     return;
   }
 
+  // consumer c: rows 64 c .. 64 c + 63 of the tile and of its staging tile
   const int c = wg - 1;
   const int t = threadIdx.x & 127;
-  float acc[BN / 2];
-#pragma unroll
-  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-  const uint32_t ab0 = smem_u32(smem_ab);
-  for (int kb = 0; kb < num_kb; ++kb) {
-    const int s = kb % kStages;
-    mbar_wait_quiet(&full[s], (kb / kStages) & 1);
-    const uint32_t sa = ab0 + s * Cfg::kStageBytes + c * (64 * 128);
-    const uint32_t sw = ab0 + s * Cfg::kStageBytes + Cfg::kABytes;
-    wgmma_fence();
-#pragma unroll
-    for (int k = 0; k < kBK / 16; ++k) wgmma_tile<BN>(acc, wgmma_desc_sw128(sa + 32 * k), wgmma_desc_sw128(sw + 32 * k), 1u);
-    wgmma_commit();
-    wgmma_wait<1>();  // the group of k-block kb - 1 has retired: its stage can be refilled
-    if (kb > 0 && t == 0) mbar_arrive(&empty[(kb - 1) % kStages]);
-  }
+  float acc[1][BN / 2];
+  consumer_k_loop<Cfg, 1>(acc, smem_u32(smem_ab), c * (64 * 128), full, empty, 0, num_kb, t);
   wgmma_wait<0>();
-
-  const int warp = t >> 5, lane = t & 31;
-  const int rl0 = c * 64 + warp * 16 + (lane >> 2);  // tile rows of acc[.. 0/1] and (+8) acc[.. 2/3]
-#pragma unroll
-  for (int j = 0; j < BN / 8; ++j) {
-    const int col = j * 8 + 2 * (lane & 3);  // column inside the tile
-    const int gcol = n0 + col;
-    float2 b2 = make_float2(0.f, 0.f);
-    if (bias != nullptr && gcol < N) b2 = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(bias + gcol)));
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int row = rl0 + 8 * h;
-      float x0 = acc[4 * j + 2 * h] + b2.x, x1 = acc[4 * j + 2 * h + 1] + b2.y;
-      if (ACT == 1) {
-        x0 = gelu_tanh_f(rbf(x0));
-        x1 = gelu_tanh_f(rbf(x1));
-      }
-      unsigned char* dst = smem_c + (col >> 6) * (kBM * 128) + row * 128 + ((((col & 63) >> 3) ^ (row & 7)) << 4) + (col & 7) * 2;
-      *reinterpret_cast<uint32_t*>(dst) = pack_bf16x2(x0, x1);  // ACT 3: the rounded pre-activation, see below
-    }
-  }
-  if (ACT == 3) {
-    // erf-GELU in a second pass over the thread's own staging slots, once the accumulators are dead: erff next to the
-    // live accumulators would not fit in the register budget.  The slot holds rbf(x), the value the GELU is evaluated
-    // on; the empty asm makes the compiler reload it rather than carry the first pass's registers over.
-    asm volatile("" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < BN / 4; ++i) {
-      const int col = (i >> 1) * 8 + 2 * (lane & 3), row = rl0 + 8 * (i & 1);
-      uint32_t* dst = reinterpret_cast<uint32_t*>(smem_c + (col >> 6) * (kBM * 128) + row * 128 +
-                                                  ((((col & 63) >> 3) ^ (row & 7)) << 4) + (col & 7) * 2);
-      const float2 v = unpack_bf16x2(*dst);
-      *dst = pack_bf16x2(gelu_erf_f(v.x), gelu_erf_f(v.y));
-    }
-  }
+  gemm_epilogue<BN, 1, ACT>(acc, smem_u32(smem_c) + c * (64 * 128), m0 + 64 * c, n0, M, N, bias, ep, nullptr, 0, t >> 5,
+                            t & 31);
   fence_proxy_async_smem();
   named_bar_sync(1, 256);
   if (threadIdx.x == 128) {
@@ -281,42 +308,9 @@ gemm_tile_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant
   }
 }
 
-template <int BN, int ACT>
-static int launch_gemm_tile(const void* A, const void* W, const bf16* bias, void* out, int M, int N, int K,
-                            const CUtensorMap& ta, cudaStream_t st) {
-  static bool attr = false;
-  if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_tile_kernel<BN, ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         TileCfg<BN>::kSmemBytes);
-    if (e != cudaSuccess) return fail(VSB_ERR_CUDA, "gemm: smem attr: %s", cudaGetErrorString(e));
-    attr = true;
-  }
-  CUtensorMap tw, tc;
-  unsigned long long dw[2] = {(unsigned long long)K, (unsigned long long)N};
-  unsigned long long sw[1] = {(unsigned long long)K * 2};
-  unsigned bw[2] = {kBK, (unsigned)BN};
-  int rc = make_tmap_bf16(&tw, W, 2, dw, sw, bw, CU_TENSOR_MAP_SWIZZLE_128B);
-  if (rc) return rc;
-  unsigned long long dc[2] = {(unsigned long long)N, (unsigned long long)M};
-  unsigned long long sc[1] = {(unsigned long long)N * 2};
-  unsigned bc[2] = {64, kBM};
-  rc = make_tmap_bf16(&tc, out, 2, dc, sc, bc, CU_TENSOR_MAP_SWIZZLE_128B);
-  if (rc) return rc;
-  const long long tiles = (long long)((M + kBM - 1) / kBM) * ((N + BN - 1) / BN);
-  gemm_tile_kernel<BN, ACT><<<(unsigned)tiles, kTileThreads, TileCfg<BN>::kSmemBytes, st>>>(ta, tw, tc, bias, M, N, K);
-  return check_launch("gemm_tile");
-}
-
 // ---- persistent ping-pong kernel: the epilogues that cost (gate + residual, GELU at short K) ------------------------
-// TMA store from a 32-bit shared-memory address (the consumers keep no 64-bit pointer live across the mainloop)
-__device__ __forceinline__ void tma_store_2d_s(const CUtensorMap* m, uint32_t src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(reinterpret_cast<uint64_t>(m)),
-               "r"(src), "r"(c0), "r"(c1)
-               : "memory");
-}
-
 template <int ACT>
-__global__ void __launch_bounds__(kGemmThreads, 1)
+__global__ void __launch_bounds__(GemmCfg::kThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_w,
                   const __grid_constant__ CUtensorMap tm_c, const __grid_constant__ CUtensorMap tm_r,
                   const bf16* __restrict__ bias, int M, int N, int K, const EpiArgs ep) {
@@ -361,12 +355,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
       for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x, ++j) {
         const int m0 = (tile / tiles_n) * kBM, n0 = (tile % tiles_n) * kBN;
         for (int kb = 0; kb < num_kb; ++kb, ++n) {
-          const int s = n % kStages;
-          mbar_wait_quiet(&empty[s], ((n / kStages) & 1) ^ 1);
-          unsigned char* sa = smem_ab + s * Cfg::kStageBytes;
-          mbar_arrive_expect_tx(&full[s], Cfg::kStageBytes);
-          tma_load_2d(&tm_a, &full[s], sa, kb * kBK, m0);
-          tma_load_2d(&tm_w, &full[s], sa + Cfg::kABytes, kb * kBK, n0);
+          load_k_block<Cfg>(&tm_a, &tm_w, smem_ab, full, empty, n, kb, m0, n0, 1);
           if (ACT == 2 && kb == min(kStages, num_kb) - 1) {
             // the resid block, once the ring holds the tile's first k-blocks: the consumer is done with its previous
             // tile's staging by the time it needs more of this tile's k-blocks
@@ -393,34 +382,14 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
   for (int j = c, tile = blockIdx.x + c * gridDim.x; tile < tiles; j += 2, tile += 2 * gridDim.x, ++u) {
     const int m0 = (tile / tiles_n) * kBM, n0 = (tile % tiles_n) * kBN;
     float acc[2][64];
-#pragma unroll
-    for (int h = 0; h < 2; ++h)
-#pragma unroll
-      for (int i = 0; i < 64; ++i) acc[h][i] = 0.f;
-
     if (j > 0) named_bar_sync(1 + c, 256);  // our turn: the other consumer has issued its mainloop of tile j - 1
     const int n_base = j * num_kb;          // ring position of this tile's first k-block
-    for (int kb = 0; kb < num_kb; ++kb) {
-      const int n = n_base + kb, s = n % kStages;
-      mbar_wait_quiet(&full[s], (n / kStages) & 1);
-      const uint32_t sa = ab0 + s * Cfg::kStageBytes;
-      const uint32_t sw = sa + Cfg::kABytes;
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < kBK / 16; ++k) {
-        const uint64_t dw = wgmma_desc_sw128(sw + 32 * k);
-        wgmma_m64n128k16_ss(acc[0], wgmma_desc_sw128(sa + 32 * k), dw, 1u);
-        wgmma_m64n128k16_ss(acc[1], wgmma_desc_sw128(sa + 64 * 128 + 32 * k), dw, 1u);
-      }
-      wgmma_commit();
-      wgmma_wait<1>();  // the group of k-block kb - 1 has retired: its stage can be refilled
-      if (kb > 0 && t == 0) mbar_arrive(&empty[(n - 1) % kStages]);
-    }
+    consumer_k_loop<Cfg, 2>(acc, ab0, 0, full, empty, n_base, num_kb, t);
     if (tile + gridDim.x < tiles) named_bar_arrive(1 + (c ^ 1), 256);  // hand the tensor cores to tile j + 1
     wgmma_wait<0>();
     if (t == 0) mbar_arrive(&empty[(n_base + num_kb - 1) % kStages]);
 
-    gemm_epilogue<ACT>(acc, my_c, m0, n0, M, N, bias, ep, &c_full[c], u & 1, warp, lane);
+    gemm_epilogue<kBN, 2, ACT>(acc, my_c, m0, n0, M, N, bias, ep, &c_full[c], u & 1, warp, lane);
     fence_proxy_async_smem();
     named_bar_sync(3 + c, 128);
     if (t == 0) {
@@ -437,22 +406,6 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
   if (t == 0) tma_store_wait0();
 }
 
-template <int ACT>
-static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tw, const CUtensorMap& tc, const CUtensorMap& tr,
-                       const bf16* bias, int M, int N, int K, cudaStream_t st, const EpiArgs& ep) {
-  static bool attr = false;
-  if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_wgmma_kernel<ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         GemmCfg::kSmemBytes);
-    if (e != cudaSuccess) return fail(VSB_ERR_CUDA, "gemm: smem attr: %s", cudaGetErrorString(e));
-    attr = true;
-  }
-  const long long tiles = (long long)((M + kBM - 1) / kBM) * ((N + kBN - 1) / kBN);
-  const int grid = tiles < num_sms() ? int(tiles) : num_sms();
-  gemm_wgmma_kernel<ACT><<<grid, kGemmThreads, GemmCfg::kSmemBytes, st>>>(ta, tw, tc, tr, bias, M, N, K, ep);
-  return check_launch("gemm_wgmma");
-}
-
 // ---- persistent cooperative kernel on 256 x 128 tiles: the large-M Linears --------------------------------------------
 // min(tiles, SMs) CTAs walk the 256 x 128 output tiles with a static stride, N-fastest.  Both consumer warpgroups work on
 // the same tile, warpgroup c on rows 128 c .. 128 c + 127, with the same 2 x wgmma.m64n128k16 per k16 step as a consumer
@@ -460,29 +413,16 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tw, const CUten
 // fewer L2 -> SM bytes per FLOP than the 128 x 128 tile.
 // Without a second tile to ping-pong with, the epilogue is split so that little of it stays off the tensor cores.  Every
 // epilogue starts from y = bf16(acc + bias): the consumers store that into their half of the staging tile (the bias-only
-// epilogue of gemm_epilogue) and go on to the next tile's mainloop; three epilogue warps then apply the rest in place --
-// tanh-GELU(y), erf-GELU(y), or resid + [bf16(gate * y)] with resid read from global memory -- and TMA-store the tile.
-// Every step sees the same 16-bit y and does the same fp32 arithmetic as in gemm_wgmma_kernel, so the outputs are
+// gemm_epilogue) and go on to the next tile's mainloop; three epilogue warps then apply the rest in place -- tanh-GELU(y),
+// erf-GELU(y), or resid + [bf16(gate * y)] with resid read from global memory -- and TMA-store the tile.
+// Every step sees the same 16-bit y and calls the same element functions as gemm_wgmma_kernel, so the outputs are
 // bit-identical.  Barriers per staging half c: st_full[c] (the consumer's 128 threads have written y), st_free[c] (the
 // tile's TMA store has read the half).
-constexpr int kWideThreads = 384;  // two consumer warpgroups, three epilogue warps, one producer warp
-constexpr int kWideEpiThreads = 96;
-
-struct WideCfg {
-  static constexpr int kBMw = 2 * kBM;
-  static constexpr int kABytes = kBMw * kBK * 2;  // two 128-row TMA boxes
-  static constexpr int kStageBytes = kABytes + kBN * kBK * 2;
-  static constexpr int kCBytes = kBM * kBN * 2;  // one consumer's half of the staging tile
-  static constexpr int kStages = 3;
-  // 3 x 48 KB ring + 2 x 32 KB staging, + 1024 for manual alignment, + 256 for barriers: 214 272 B of the 227 KB
-  static constexpr int kSmemBytes = kStages * kStageBytes + 2 * kCBytes + 1024 + 256;
-};
-
 template <int ACT>
-__global__ void __launch_bounds__(kWideThreads, 1)
+__global__ void __launch_bounds__(WideCfg::kThreads, 1)
 gemm_wide_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_w,
-                 const __grid_constant__ CUtensorMap tm_c, const bf16* __restrict__ bias, int M, int N, int K,
-                 const EpiArgs ep) {
+                 const __grid_constant__ CUtensorMap tm_c, const __grid_constant__ CUtensorMap tm_r,
+                 const bf16* __restrict__ bias, int M, int N, int K, const EpiArgs ep) {
   using Cfg = WideCfg;
   constexpr int kStages = Cfg::kStages;
   extern __shared__ unsigned char smem_dyn[];
@@ -496,7 +436,7 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant
 
   const int wg = threadIdx.x >> 7;
   const int tiles_n = (N + kBN - 1) / kBN;
-  const int tiles = ((M + Cfg::kBMw - 1) / Cfg::kBMw) * tiles_n;
+  const int tiles = ((M + Cfg::kTileM - 1) / Cfg::kTileM) * tiles_n;
   const int num_kb = (K + kBK - 1) / kBK;
 
   if (threadIdx.x == 0) {
@@ -520,17 +460,9 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant
       // ===================== TMA producer (warp 11) =====================
       int n = 0;  // k-blocks loaded so far: the position in the ring, carried over between tiles
       for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
-        const int m0 = (tile / tiles_n) * Cfg::kBMw, n0 = (tile % tiles_n) * kBN;
-        const bool lower = m0 + kBM < M;  // the lower half has rows inside M (else its A loads are skipped)
-        for (int kb = 0; kb < num_kb; ++kb, ++n) {
-          const int s = n % kStages;
-          mbar_wait_quiet(&empty[s], ((n / kStages) & 1) ^ 1);
-          unsigned char* sa = smem_ab + s * Cfg::kStageBytes;
-          mbar_arrive_expect_tx(&full[s], Cfg::kStageBytes - (lower ? 0 : kBM * kBK * 2));
-          tma_load_2d(&tm_a, &full[s], sa, kb * kBK, m0);
-          if (lower) tma_load_2d(&tm_a, &full[s], sa + kBM * kBK * 2, kb * kBK, m0 + kBM);
-          tma_load_2d(&tm_w, &full[s], sa + Cfg::kABytes, kb * kBK, n0);
-        }
+        const int m0 = (tile / tiles_n) * Cfg::kTileM, n0 = (tile % tiles_n) * kBN;
+        const int a_boxes = m0 + kBM < M ? 2 : 1;  // the lower half's A box only where it has rows inside M
+        for (int kb = 0; kb < num_kb; ++kb, ++n) load_k_block<Cfg>(&tm_a, &tm_w, smem_ab, full, empty, n, kb, m0, n0, a_boxes);
       }
     } else if (threadIdx.x < 256 + kWideEpiThreads) {
       // ===================== epilogue warps 8-10: the staged y -> the output, under the next mainloop ===============
@@ -538,7 +470,7 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant
       const uint32_t c0 = smem_u32(smem_c);
       int j = 0;
       for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x, ++j) {
-        const int m0 = (tile / tiles_n) * Cfg::kBMw, n0 = (tile % tiles_n) * kBN;
+        const int m0 = (tile / tiles_n) * Cfg::kTileM, n0 = (tile % tiles_n) * kBN;
         mbar_wait_quiet(&st_full[0], j & 1);
         mbar_wait_quiet(&st_full[1], j & 1);
         if (ACT != 0) {
@@ -558,28 +490,19 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant
               const uint32_t r[4] = {r4.x, r4.y, r4.z, r4.w};
               uint32_t g[4] = {0, 0, 0, 0};
               if (ep.gate_row >= 0) {
-                const int bt = grow / ep.S;
-                const int bb = bt / ep.T;
-                const int sel = (ep.x_mask != nullptr && ep.x_mask[bt] == 0) ? 1 : 0;
-                const uint4 g4 = __ldg(reinterpret_cast<const uint4*>(ep.mod + ((sel * ep.B + bb) * 6 + ep.gate_row) * N + gcol));
+                const uint4 g4 = __ldg(reinterpret_cast<const uint4*>(ep.mod + (gate_offset(ep, grow, N) + gcol)));
                 g[0] = g4.x, g[1] = g4.y, g[2] = g4.z, g[3] = g4.w;
               }
 #pragma unroll
               for (int i = 0; i < 4; ++i) {
-                float2 y = unpack_bf16x2(v[i]);  // the Linear's 16-bit output
-                if (ep.gate_row >= 0) {
-                  const float2 gg = unpack_bf16x2(g[i]);
-                  y.x = rbf(gg.x * y.x);  // bf16(gate * y)
-                  y.y = rbf(gg.y * y.y);
-                }
-                const float2 xr = unpack_bf16x2(r[i]);
-                v[i] = pack_bf16x2(xr.x + y.x, xr.y + y.y);  // residual add, rounded by the pack
+                const float2 x = residual_add2(unpack_bf16x2(v[i]), r[i], ep.gate_row >= 0, g[i]);
+                v[i] = pack_bf16x2(x.x, x.y);
               }
             } else {
 #pragma unroll
               for (int i = 0; i < 4; ++i) {
-                const float2 y = unpack_bf16x2(v[i]);
-                v[i] = ACT == 1 ? pack_bf16x2(gelu_tanh_f(y.x), gelu_tanh_f(y.y)) : pack_bf16x2(gelu_erf_f(y.x), gelu_erf_f(y.y));
+                const float2 x = gelu2<ACT>(unpack_bf16x2(v[i]));
+                v[i] = pack_bf16x2(x.x, x.y);
               }
             }
             asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3])
@@ -613,57 +536,85 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant
   const uint32_t ab0 = smem_u32(smem_ab);
   int j = 0;
   for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x, ++j) {
-    const int m0 = (tile / tiles_n) * Cfg::kBMw + c * kBM, n0 = (tile % tiles_n) * kBN;
+    const int m0 = (tile / tiles_n) * Cfg::kTileM + c * kBM, n0 = (tile % tiles_n) * kBN;
     float acc[2][64];
-#pragma unroll
-    for (int h = 0; h < 2; ++h)
-#pragma unroll
-      for (int i = 0; i < 64; ++i) acc[h][i] = 0.f;
-
     const int n_base = j * num_kb;  // ring position of this tile's first k-block
-    for (int kb = 0; kb < num_kb; ++kb) {
-      const int n = n_base + kb, s = n % kStages;
-      mbar_wait_quiet(&full[s], (n / kStages) & 1);
-      const uint32_t sa = ab0 + s * Cfg::kStageBytes + c * (kBM * kBK * 2);
-      const uint32_t sw = ab0 + s * Cfg::kStageBytes + Cfg::kABytes;
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < kBK / 16; ++k) {
-        const uint64_t dw = wgmma_desc_sw128(sw + 32 * k);
-        wgmma_m64n128k16_ss(acc[0], wgmma_desc_sw128(sa + 32 * k), dw, 1u);
-        wgmma_m64n128k16_ss(acc[1], wgmma_desc_sw128(sa + 64 * 128 + 32 * k), dw, 1u);
-      }
-      wgmma_commit();
-      wgmma_wait<1>();  // the group of k-block kb - 1 has retired: its stage can be refilled
-      if (kb > 0 && t == 0) mbar_arrive(&empty[(n - 1) % kStages]);
-    }
+    consumer_k_loop<Cfg, 2>(acc, ab0, c * kABox, full, empty, n_base, num_kb, t);
     wgmma_wait<0>();
     if (t == 0) mbar_arrive(&empty[(n_base + num_kb - 1) % kStages]);
 
     if (j > 0) mbar_wait_quiet(&st_free[c], (j - 1) & 1);  // the previous tile's store has read this half
-    gemm_epilogue<0>(acc, my_c, m0, n0, M, N, bias, ep, nullptr, 0, warp, lane);  // y = bf16(acc + bias)
+    gemm_epilogue<kBN, 2, 0>(acc, my_c, m0, n0, M, N, bias, ep, nullptr, 0, warp, lane);  // y = bf16(acc + bias)
     fence_proxy_async_smem();  // bias only: the TMA store reads y as written
     mbar_arrive(&st_full[c]);
   }
 }
 
-template <int ACT>
-static int launch_gemm_wide(const CUtensorMap& ta, const CUtensorMap& tw, const CUtensorMap& tc, const bf16* bias, int M,
-                            int N, int K, cudaStream_t st, const EpiArgs& ep) {
+// ---- host side ---------------------------------------------------------------------------------------------------------
+// Tensor map of a row-major [rows, cols] 16-bit matrix, moved in 128B-swizzled boxes of box_rows x 64 columns.
+static int make_tmap_rows(CUtensorMap* m, const void* p, int rows, int cols, int box_rows) {
+  const unsigned long long dims[2] = {(unsigned long long)cols, (unsigned long long)rows};
+  const unsigned long long stride[1] = {(unsigned long long)cols * 2};
+  const unsigned box[2] = {64, (unsigned)box_rows};
+  return make_tmap_bf16(m, p, 2, dims, stride, box, CU_TENSOR_MAP_SWIZZLE_128B);
+}
+
+typedef int (*GemmLaunch)(const void* A, const void* W, const bf16* bias, void* out, int M, int N, int K,
+                          const EpiArgs& ep, cudaStream_t st);
+
+// Launches one kernel instance: a CTA per tile, or min(tiles, SMs) CTAs for a persistent kernel.  The first launch of
+// an instance raises its dynamic shared-memory limit.  All three kernels take the same parameters, so that this one
+// launcher serves them; tm_r (read only by gemm_wgmma_kernel<2>) and ep go unused where the epilogue has no residual.
+template <auto kKernel, class Cfg>
+static int launch_gemm(const void* A, const void* W, const bf16* bias, void* out, int M, int N, int K,
+                       const EpiArgs& ep, cudaStream_t st) {
   static bool attr = false;
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_wide_kernel<ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         WideCfg::kSmemBytes);
+    cudaError_t e = cudaFuncSetAttribute(kKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
     if (e != cudaSuccess) return fail(VSB_ERR_CUDA, "gemm: smem attr: %s", cudaGetErrorString(e));
     attr = true;
   }
-  const long long tiles = (long long)((M + WideCfg::kBMw - 1) / WideCfg::kBMw) * ((N + kBN - 1) / kBN);
-  const int grid = tiles < num_sms() ? int(tiles) : num_sms();
-  gemm_wide_kernel<ACT><<<grid, kWideThreads, WideCfg::kSmemBytes, st>>>(ta, tw, tc, bias, M, N, K, ep);
-  return check_launch("gemm_wide");
+  CUtensorMap ta, tw, tc, tr;
+  int rc = make_tmap_rows(&ta, A, M, K, kBM);
+  if (!rc) rc = make_tmap_rows(&tw, W, N, K, Cfg::kTileN);
+  if (!rc) rc = make_tmap_rows(&tc, out, M, N, kBM);
+  if (rc) return rc;
+  tr = tc;  // unused without a resid
+  if (ep.resid != nullptr) {
+    rc = make_tmap_rows(&tr, ep.resid, M, N, kBM);
+    if (rc) return rc;
+  }
+  const long long tiles = (long long)((M + Cfg::kTileM - 1) / Cfg::kTileM) * ((N + Cfg::kTileN - 1) / Cfg::kTileN);
+  const int grid = Cfg::kPersistent && tiles > num_sms() ? num_sms() : int(tiles);
+  kKernel<<<grid, Cfg::kThreads, Cfg::kSmemBytes, st>>>(ta, tw, tc, tr, bias, M, N, K, ep);
+  return check_launch("gemm");
 }
 
 enum class GemmKernel { kTile128, kTile192, kPingPong, kWide };
+
+// The instance gemm_dispatch launches and vsb_gemm_kernel_name reports, by [GemmKernel][epilogue]; an empty slot is one
+// gemm_route never picks.
+struct GemmInstance {
+  GemmLaunch launch;
+  const char* name;
+};
+static const GemmInstance kGemmInstances[4][4] = {
+    {{launch_gemm<gemm_tile_kernel<128, 0>, TileCfg<128>>, "gemm_tile_kernel<128, 0>"},
+     {launch_gemm<gemm_tile_kernel<128, 1>, TileCfg<128>>, "gemm_tile_kernel<128, 1>"},
+     {},
+     {launch_gemm<gemm_tile_kernel<128, 3>, TileCfg<128>>, "gemm_tile_kernel<128, 3>"}},
+    {{launch_gemm<gemm_tile_kernel<192, 0>, TileCfg<192>>, "gemm_tile_kernel<192, 0>"},
+     {launch_gemm<gemm_tile_kernel<192, 1>, TileCfg<192>>, "gemm_tile_kernel<192, 1>"},
+     {},
+     {launch_gemm<gemm_tile_kernel<192, 3>, TileCfg<192>>, "gemm_tile_kernel<192, 3>"}},
+    {{},
+     {launch_gemm<gemm_wgmma_kernel<1>, GemmCfg>, "gemm_wgmma_kernel<1>"},
+     {launch_gemm<gemm_wgmma_kernel<2>, GemmCfg>, "gemm_wgmma_kernel<2>"},
+     {launch_gemm<gemm_wgmma_kernel<3>, GemmCfg>, "gemm_wgmma_kernel<3>"}},
+    {{launch_gemm<gemm_wide_kernel<0>, WideCfg>, "gemm_wide_kernel<0>"},
+     {launch_gemm<gemm_wide_kernel<1>, WideCfg>, "gemm_wide_kernel<1>"},
+     {launch_gemm<gemm_wide_kernel<2>, WideCfg>, "gemm_wide_kernel<2>"},
+     {launch_gemm<gemm_wide_kernel<3>, WideCfg>, "gemm_wide_kernel<3>"}}};
 
 // Which kernel runs a GEMM; act: 0 none, 1 tanh-GELU, 2 fused residual, 3 erf-GELU.
 static GemmKernel gemm_route(int M, int N, int K, int act) {
@@ -675,7 +626,7 @@ static GemmKernel gemm_route(int M, int N, int K, int act) {
   //   erf-GELU, K 2304: 1.09x;  gate + residual (was persistent): K 1152 0.55x, K 4608 1.24x
   // The residual epilogue reads resid from global memory in the epilogue warps, which a K loop of 1152 does not hide.
   // It runs at 2048 tiles or more: the fewest it was measured at (CogVideoX-2B, 2085).
-  const long long wide_tiles = (long long)((M + WideCfg::kBMw - 1) / WideCfg::kBMw) * ((N + kBN - 1) / kBN);
+  const long long wide_tiles = (long long)((M + WideCfg::kTileM - 1) / WideCfg::kTileM) * ((N + kBN - 1) / kBN);
   if (wide_tiles >= kWideMinTiles && (act != 2 || K >= 4608))
     return GemmKernel::kWide;
   // The persistent kernel's K loop is slower than the one-tile-per-CTA kernel's (0.671 against 0.521 ms per 1152 of K at
@@ -690,61 +641,15 @@ static GemmKernel gemm_route(int M, int N, int K, int act) {
   return GemmKernel::kPingPong;
 }
 
-static const char* gemm_kernel_name(GemmKernel k, int act) {
-  static const char* const names[4][4] = {
-      {"gemm_tile_kernel<128, 0>", "gemm_tile_kernel<128, 1>", "", "gemm_tile_kernel<128, 3>"},
-      {"gemm_tile_kernel<192, 0>", "gemm_tile_kernel<192, 1>", "", "gemm_tile_kernel<192, 3>"},
-      {"", "gemm_wgmma_kernel<1>", "gemm_wgmma_kernel<2>", "gemm_wgmma_kernel<3>"},
-      {"gemm_wide_kernel<0>", "gemm_wide_kernel<1>", "gemm_wide_kernel<2>", "gemm_wide_kernel<3>"}};
-  return names[int(k)][act];
-}
-
 // act: 0 none, 1 tanh-GELU, 2 fused residual (ep->resid != nullptr), 3 erf-GELU
 static int gemm_dispatch(const void* A, const void* W, const void* bias, void* out, int M, int N, int K, int act,
                          cudaStream_t st, const EpiArgs& ep) {
   if ((long long)((M + kBM - 1) / kBM) * ((N + kBN - 1) / kBN) > 0x7fffffffLL)
     return fail(VSB_ERR_UNSUPPORTED, "gemm: too many tiles (M=%d N=%d)", M, N);
-  CUtensorMap ta, tw, tc, tr;
-  unsigned long long da[2] = {(unsigned long long)K, (unsigned long long)M};
-  unsigned long long sa[1] = {(unsigned long long)K * 2};
-  unsigned ba[2] = {kBK, kBM};
-  int rc = make_tmap_bf16(&ta, A, 2, da, sa, ba, CU_TENSOR_MAP_SWIZZLE_128B);
-  if (rc) return rc;
-  const bf16* b = (const bf16*)bias;
   const GemmKernel kern = gemm_route(M, N, K, act);
-  if (kern == GemmKernel::kTile128 || kern == GemmKernel::kTile192) {
-#define VSB_TILE_CASE(a)                                                                                      \
-  if (act == a) return kern == GemmKernel::kTile192 ? launch_gemm_tile<192, a>(A, W, b, out, M, N, K, ta, st) \
-                                                    : launch_gemm_tile<128, a>(A, W, b, out, M, N, K, ta, st);
-    VSB_TILE_CASE(0)
-    VSB_TILE_CASE(1)
-    VSB_TILE_CASE(3)
-#undef VSB_TILE_CASE
-  }
-  unsigned long long dw[2] = {(unsigned long long)K, (unsigned long long)N};
-  unsigned bw[2] = {kBK, (unsigned)kBN};
-  rc = make_tmap_bf16(&tw, W, 2, dw, sa, bw, CU_TENSOR_MAP_SWIZZLE_128B);
-  if (rc) return rc;
-  unsigned long long dc[2] = {(unsigned long long)N, (unsigned long long)M};
-  unsigned long long sc[1] = {(unsigned long long)N * 2};
-  unsigned bc[2] = {64, kBM};
-  rc = make_tmap_bf16(&tc, out, 2, dc, sc, bc, CU_TENSOR_MAP_SWIZZLE_128B);
-  if (rc) return rc;
-  if (act == 2) {
-    rc = make_tmap_bf16(&tr, ep.resid, 2, dc, sc, bc, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (rc) return rc;
-  } else {
-    tr = tc;  // unused
-  }
-  if (kern == GemmKernel::kWide) {
-    if (act == 0) return launch_gemm_wide<0>(ta, tw, tc, b, M, N, K, st, ep);
-    if (act == 1) return launch_gemm_wide<1>(ta, tw, tc, b, M, N, K, st, ep);
-    if (act == 2) return launch_gemm_wide<2>(ta, tw, tc, b, M, N, K, st, ep);
-    return launch_gemm_wide<3>(ta, tw, tc, b, M, N, K, st, ep);
-  }
-  if (act == 3) return launch_gemm<3>(ta, tw, tc, tr, b, M, N, K, st, ep);
-  if (act == 2) return launch_gemm<2>(ta, tw, tc, tr, b, M, N, K, st, ep);
-  return launch_gemm<1>(ta, tw, tc, tr, b, M, N, K, st, ep);
+  const GemmInstance& g = kGemmInstances[int(kern)][act];
+  if (g.launch == nullptr) return fail(VSB_ERR_UNSUPPORTED, "gemm: no kernel instance for route %d, epilogue %d", int(kern), act);
+  return g.launch(A, W, (const bf16*)bias, out, M, N, K, ep, st);
 }
 
 }  // namespace vsb
@@ -781,6 +686,7 @@ extern "C" int VSB_API(vsb_gemm_bias_residual)(const vsb_bf16* A, const vsb_bf16
 extern "C" const char* vsb_gemm_kernel_name(int M, int N, int K, int act, int residual) {
   if (M <= 0 || N <= 0 || K <= 0 || act < 0 || act > 2 || (residual && act != 0)) return "";
   const int epi = residual ? 2 : (act == 2 ? 3 : act);
-  return gemm_kernel_name(gemm_route(M, N, K, epi), epi);
+  const char* name = kGemmInstances[int(gemm_route(M, N, K, epi))][epi].name;
+  return name != nullptr ? name : "";
 }
 #endif
