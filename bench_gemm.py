@@ -20,6 +20,13 @@
                one-tile-per-CTA kernel's GELU epilogues (K 2304) at tile widths 192 and 128, and its 128-wide bias-only
                tile (n1024, K 1152)
 
+FP8 twins (``<name>_fp8``) of the six OpenSora 720p Linears run ``kernels.gemm_fp8_bias_act`` / ``_residual`` on e4m3
+operands with the same epilogue; where the FP8 mode of the model quantizes the input in a pass of its own (attn_proj,
+q_linear, cross_proj, fc2) that pass (``kernels.quant_rows_fp8``) is inside the timed launch, so their rate is FLOPs
+over quantization + GEMM.  qkv and fc1 take their codes from the modulate kernel.  ``quant_k1152`` / ``quant_k4608``
+time the quantization alone at M = 2 x 20 x 3600, as bytes (2 B read + 1 B written per element, 4 B per row) against
+3.35 TB/s.
+
     python bench_gemm.py [--iters 20] [--warmup 3] [--rounds 3] [--shapes a,b] [--no-cublas] [--out FILE.json]
 
 Inputs are seeded, so two builds given the same arguments can be compared output for output: every shape prints the
@@ -69,6 +76,15 @@ SHAPES = {
     "n1024_tanh": (4096, 1024, 2304, torch.bfloat16, 1),
     "n1024_erf": (4096, 1024, 2304, torch.bfloat16, 2),
 }
+# name: (the bf16 shape, whether the timed launch includes the activation's quantization)
+FP8_SHAPES = {"qkv_fp8": ("qkv", False), "attn_proj_fp8": ("attn_proj", True), "q_linear_fp8": ("q_linear", True),
+              "cross_proj_fp8": ("cross_proj", True), "fc1_fp8": ("fc1", False), "fc2_fp8": ("fc2", True)}
+QUANT_SHAPES = {"quant_k1152": (M720, 1152), "quant_k4608": (M720, 4608)}
+HBM_BYTES_PER_S = 3.35e12
+for _n, (_b, _) in FP8_SHAPES.items():
+    SHAPES[_n] = SHAPES[_b]
+for _n, (_m, _k) in QUANT_SHAPES.items():
+    SHAPES[_n] = (_m, _k, _k, torch.bfloat16, "quant")
 B720, T720, S720 = 2, 20, 3600
 
 
@@ -86,6 +102,22 @@ def make_call(name, dev, seed):
     def cublas():
         torch.nn.functional.linear(a, w, bias)
 
+    if epi == "quant":
+        res = []
+
+        def launch():
+            res[:] = kernels.quant_rows_fp8(a)
+        launch()
+        return launch, (lambda: None), lambda: res[0], cublas, 3 * M * K + 4 * M
+    fp8 = name in FP8_SHAPES
+    if fp8:
+        wq, ws = kernels.quant_rows_fp8(w)
+        aq = kernels.quant_rows_fp8(a)
+        with_quant = FP8_SHAPES[name][1]
+
+        def gemm_a():
+            return kernels.quant_rows_fp8(a) if with_quant else aq
+
     if isinstance(epi, tuple):
         gate_row = epi[1]
         x0 = rnd(M, N)
@@ -96,7 +128,10 @@ def make_call(name, dev, seed):
         mask[1, 17] = 0
 
         def launch():
-            if gate_row >= 0:
+            if fp8:
+                kernels.gemm_fp8_bias_residual(*gemm_a(), wq, ws, bias, x, *((mod, mask, gate_row, B720, T720, S720)
+                                                                              if gate_row >= 0 else ()))
+            elif gate_row >= 0:
                 kernels.gemm_bias_residual(a, w, bias, x, mod, mask, gate_row, B720, T720, S720)
             else:
                 kernels.gemm_bias_residual(a, w, bias, x)
@@ -107,7 +142,10 @@ def make_call(name, dev, seed):
     out = torch.empty(M, N, device=dev, dtype=dt)
 
     def launch():
-        kernels.gemm_bias_act(a, w, bias, act=epi, out=out)
+        if fp8:
+            kernels.gemm_fp8_bias_act(*gemm_a(), wq, ws, bias, act=epi, out=out)
+        else:
+            kernels.gemm_bias_act(a, w, bias, act=epi, out=out)
     return launch, (lambda: None), out, cublas, 2 * M * N * K
 
 
@@ -140,6 +178,11 @@ def kernel_of(name):
     from videosys_b200 import kernels
 
     M, N, K, _, epi = SHAPES[name]
+    if epi == "quant":
+        return "quant_rows_fp8_kernel"
+    if name in FP8_SHAPES:
+        q = "quant_rows_fp8_kernel + " if FP8_SHAPES[name][1] else ""
+        return q + kernels.gemm_fp8_kernel_name(M, N, K, act=0 if isinstance(epi, tuple) else epi, residual=isinstance(epi, tuple))
     if isinstance(epi, tuple):
         return kernels.gemm_kernel_name(M, N, K, residual=True)
     return kernels.gemm_kernel_name(M, N, K, act=epi)
@@ -152,9 +195,15 @@ def run_shape(name, seed, iters, warmup, cublas):
     reset()
     launch()
     torch.cuda.synchronize()
-    digest = hashlib.sha256(out.view(torch.int16).cpu().numpy().tobytes()).hexdigest()
+    quant = SHAPES[name][4] == "quant"
+    digest = hashlib.sha256((out()[0].view(torch.uint8) if quant else out.view(torch.int16)).cpu().numpy().tobytes()).hexdigest()
     ms, mhz = _time(launch, iters, warmup)
     res = dict(ms=round(ms, 4), tflops=round(flops / (ms * 1e-3) / 1e12, 1), sha256=digest, sm_mhz=mhz)
+    if quant:  # bytes, not FLOPs: the rate is TB/s, and its share of the HBM bandwidth
+        res.update(tflops=None, tb_s=round(flops / (ms * 1e-3) / 1e12, 3), hbm_share=round(flops / (ms * 1e-3) / HBM_BYTES_PER_S, 3))
+        cublas = False
+    if name in FP8_SHAPES:
+        cublas = False
     if cublas:
         ms_ref, _ = _time(ref, iters, warmup)
         res["cublas_ms"] = round(ms_ref, 4)
@@ -185,7 +234,8 @@ def main():
         for i, name in enumerate(names):
             m = run_shape(name, a.seed + i, a.iters, a.warmup, not a.no_cublas and r == 0)
             cb = f"  cublas {m['cublas_tflops']:6.1f} TFLOP/s" if "cublas_ms" in m else ""
-            print(f"round {r} {name:11s} {kernel_of(name):25s} {m['ms']:9.4f} ms {m['tflops']:6.1f} TFLOP/s{cb}  "
+            rate = f"{m['tb_s']:6.3f} TB/s ({100 * m['hbm_share']:.0f} % of HBM)" if "tb_s" in m else f"{m['tflops']:6.1f} TFLOP/s"
+            print(f"round {r} {name:11s} {kernel_of(name):25s} {m['ms']:9.4f} ms {rate}{cb}  "
                   f"sm {m['sm_mhz']} MHz  sha256 {m['sha256']}", flush=True)
             runs.setdefault(name, []).append(m)
     res = dict(gpu=gpu_info(), iters=a.iters, rounds=a.rounds, shapes={})
@@ -195,7 +245,8 @@ def main():
         shas = sorted({m["sha256"] for m in ms})
         res["shapes"][name] = dict(M=M, N=N, K=K, kernel=kernel_of(name), ms=med, ms_min=min(m["ms"] for m in ms),
                                    ms_max=max(m["ms"] for m in ms),
-                                   tflops=round(2 * M * N * K / (med * 1e-3) / 1e12, 1), sha256=shas[0] if len(shas) == 1 else shas,
+                                   tflops=(None if SHAPES[name][4] == "quant" else round(2 * M * N * K / (med * 1e-3) / 1e12, 1)),
+                                   sha256=shas[0] if len(shas) == 1 else shas,
                                    cublas_tflops=ms[0].get("cublas_tflops"), sm_mhz=[m["sm_mhz"] for m in ms])
     ks = [(SHAPES[n][2], res["shapes"][n]["ms"]) for n in ("q_linear", "k2304", "k4608") if n in res["shapes"]]
     if len(ks) == 3:  # least-squares line of time against K at N 1152: the intercept is the per-tile cost the mainloop does not hide

@@ -156,6 +156,36 @@ int vsb_gemm_bias_residual(const vsb_bf16* A, const vsb_bf16* W, const vsb_bf16*
  * Benchmarks label their rows with it. */
 const char* vsb_gemm_kernel_name(int M, int N, int K, int act, int residual);
 
+/* ---- FP8 (e4m3) Linears: quantized activations and weights, fp32 scales -------------------------------------------
+ * The quantization rule, one definition for the kernels below and the tests' torch restatement: a row x of 16-bit values
+ * (an activation row, or a weight's output channel) has amax = max |x|.  amax > 0: q = e4m3_rn(x * s) with
+ * s = 448 / amax, both fp32 round-to-nearest-even operations (PTX cvt.rn.satfinite.e4m3x2.f32; |x * s| <= 448 rounds
+ * inside the finite range, where torch's x.to(torch.float8_e4m3fn) gives the same codes), scale = amax / 448 (fp32).
+ * amax == 0: all-zero codes, scale = 1.
+ *
+ * vsb_quant_rows_fp8: x [M, K] 16-bit -> q [M, K] e4m3 codes, scale [M] fp32.  K % 8 == 0, K <= 4608. */
+int vsb_quant_rows_fp8(const vsb_bf16* x, uint8_t* q, float* scale, int M, int K, void* stream);
+
+/* vsb_ln_modulate whose output row goes out quantized: q [B*T*S, C] e4m3 and scale [B*T*S] fp32 are exactly
+ * vsb_quant_rows_fp8 of the 16-bit rows vsb_ln_modulate would write (the amax is over the rounded outputs). */
+int vsb_ln_modulate_fp8(const vsb_bf16* x, uint8_t* q, float* scale, const vsb_bf16* mod, const uint8_t* x_mask,
+                        int shift_row, int scale_row, int B, int T, int S, int C, float eps, void* stream);
+
+/* GEMM on e4m3 operands: A [M, K] codes with per-row scales sa [M], W [N, K] codes with per-output-channel scales sw [N].
+ *   y = bf16(acc * sa[m] * sw[n] + bias[n]), evaluated as fmaf(acc * sa[m], sw[n], bias[n]) in fp32, where acc is the
+ *   fp32 sum of the e4m3 products: the tensor cores sum 128 of K at a time into a fresh fragment, which is added to fp32
+ *   registers.  From y on, act (0 none, 1 tanh-GELU) as in vsb_gemm_bias_act, and the gate + select + residual epilogue
+ *   of vsb_gemm_bias_residual (same arguments) in vsb_gemm_fp8_bias_residual.
+ *   Requirements: K % 16 == 0 (16-byte rows of codes), N % 8 == 0, 16-byte aligned A, W, sw, out and resid;
+ *   otherwise VSB_ERR_UNSUPPORTED. */
+int vsb_gemm_fp8_bias_act(const uint8_t* A, const float* sa, const uint8_t* W, const float* sw, const vsb_bf16* bias,
+                          vsb_bf16* out, int M, int N, int K, int act, void* stream);
+int vsb_gemm_fp8_bias_residual(const uint8_t* A, const float* sa, const uint8_t* W, const float* sw, const vsb_bf16* bias,
+                               const vsb_bf16* resid, vsb_bf16* out, const vsb_bf16* mod, const uint8_t* x_mask,
+                               int gate_row, int M, int N, int K, int B, int T, int S, void* stream);
+/* The kernel instance the two fp8 GEMM entries launch, e.g. "gemm_wide_kernel<fp8, 2>"; as vsb_gemm_kernel_name. */
+const char* vsb_gemm_fp8_kernel_name(int M, int N, int K, int act, int residual);
+
 /* ---- flash attention (spatial self-attention and text cross-attention) -------------------------------
  * replaces F.scaled_dot_product_attention at attentions.py:100 and :268 (bool key mask = per-batch key count).
  * q/k/v are strided views: element (b, n, h, d) at base + b*batch_stride + n*row_stride + h*D + d (strides in
@@ -401,6 +431,15 @@ int vsb_attn_short_f16(const vsb_f16* qkv, vsb_f16* out, const vsb_f16* wq, cons
                    long long tok_stride, int n, int H, int D, float eps, float scale, int flags, void* stream);
 int vsb_gemm_bias_act_f16(const vsb_f16* A, const vsb_f16* W, const vsb_f16* bias, vsb_f16* out, int M, int N, int K,
                       int act, void* stream);
+int vsb_quant_rows_fp8_f16(const vsb_f16* x, uint8_t* q, float* scale, int M, int K, void* stream);
+int vsb_ln_modulate_fp8_f16(const vsb_f16* x, uint8_t* q, float* scale, const vsb_f16* mod, const uint8_t* x_mask,
+                            int shift_row, int scale_row, int B, int T, int S, int C, float eps, void* stream);
+int vsb_gemm_fp8_bias_act_f16(const uint8_t* A, const float* sa, const uint8_t* W, const float* sw, const vsb_f16* bias,
+                              vsb_f16* out, int M, int N, int K, int act, void* stream);
+int vsb_gemm_fp8_bias_residual_f16(const uint8_t* A, const float* sa, const uint8_t* W, const float* sw,
+                                   const vsb_f16* bias, const vsb_f16* resid, vsb_f16* out, const vsb_f16* mod,
+                                   const uint8_t* x_mask, int gate_row, int M, int N, int K, int B, int T, int S,
+                                   void* stream);
 int vsb_gemm_bias_residual_f16(const vsb_f16* A, const vsb_f16* W, const vsb_f16* bias, const vsb_f16* resid,
                            vsb_f16* out, const vsb_f16* mod, const uint8_t* x_mask, int gate_row, int M, int N, int K,
                            int B, int T, int S, void* stream);

@@ -29,6 +29,11 @@ SIGNATURES = {
     "vsb_gemm_bias_act": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "vsb_gemm_bias_residual": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "vsb_gemm_kernel_name": (C.c_char_p, [_i, _i, _i, _i, _i]),
+    "vsb_quant_rows_fp8": (_i, [_vp, _vp, _vp, _i, _i, _vp]),
+    "vsb_ln_modulate_fp8": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _f, _vp]),
+    "vsb_gemm_fp8_bias_act": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
+    "vsb_gemm_fp8_bias_residual": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "vsb_gemm_fp8_kernel_name": (C.c_char_p, [_i, _i, _i, _i, _i]),
     "vsb_attn_flash": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _ll, _ll, _ll, _ll, C.POINTER(_i), _f, _vp]),
     "vsb_pab_gate": (_i, [_i, _i, _i, C.POINTER(_i), _i, _i, _i, _i]),
     "vsb_dsp_wait": (_i, [_vp, _i, _u, _vp]),
@@ -70,7 +75,8 @@ SIGNATURES = {
 # fp16 twins (include/vsb200.h "IEEE fp16 twins"): same signatures, suffix _f16
 F16_TWINS = ("vsb_ln_modulate", "vsb_ln_modulate_affine", "vsb_modulation_table", "vsb_gate_residual", "vsb_residual_add",
              "vsb_qk_rmsnorm", "vsb_qk_rmsnorm_rope", "vsb_qk_rope_halves", "vsb_qk_layernorm", "vsb_attn_short", "vsb_gemm_bias_act",
-             "vsb_gemm_bias_residual", "vsb_attn_flash", "vsb_attn_flash_strided", "vsb_patch_embed",
+             "vsb_gemm_bias_residual", "vsb_quant_rows_fp8", "vsb_ln_modulate_fp8", "vsb_gemm_fp8_bias_act",
+             "vsb_gemm_fp8_bias_residual", "vsb_attn_flash", "vsb_attn_flash_strided", "vsb_patch_embed",
              "vsb_dwconv_shuffle", "vsb_gate_residual_unshuffle", "vsb_dwconv_ffn", "vsb_kv_compress",
              "vsb_vae_conv3d", "vsb_vae_groupnorm_stats", "vsb_vae_spatial_norm_silu", "vsb_vae_upsample2x",
              "vsb_vae_groupnorm_act", "vsb_vae_upsample_linear2x", "vsb_vae_mix", "vsb_vae_attn_split", "vsb_vae_attn_softmax",

@@ -119,7 +119,7 @@ static int make_tmap_bf16_uncached(int dtype, CUtensorMap* m, const void* base, 
       if (gstr[i - 1] % 16) return fail(VSB_ERR_UNSUPPORTED, "tensor map stride %llu not a multiple of 16 bytes", (unsigned long long)gstr[i - 1]);
     }
   }
-  CUresult r = g_encode(m, dtype ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bdim,
+  CUresult r = g_encode(m, dtype == kTmapDtypeU8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : dtype ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bdim,
                         estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(VSB_ERR_CUDA, "cuTensorMapEncodeTiled failed: CUresult %d", (int)r);

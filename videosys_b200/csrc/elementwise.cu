@@ -1,6 +1,7 @@
 // vsb200 -- HBM-bound kernels of the STDiT3 block: AdaLN modulate, gate+residual, residual add, q/k RMSNorm.
 // One pass over the activation each (128-bit coalesced loads/stores, fp32 math, bf16 rounding at the eager
 // op boundaries so results track the reference's eager chain bit-for-bit wherever the reduction order allows).
+#include <cuda_fp8.h>
 #include <string.h>
 
 #include "dsp_common.cuh"
@@ -31,6 +32,71 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
+// ---- e4m3 quantization of one row held by a warp (the rule of include/vsb200.h, vsb_quant_rows_fp8) ------------------
+// amax = max |x| over the row's 16-bit values; amax > 0: q = cvt.rn.satfinite.e4m3(x * s) with s = 448 / amax (both
+// fp32, round to nearest even), scale = amax / 448; amax == 0: all-zero codes and scale 1.  |x * s| <= 448 (1 + 2^-23)
+// rounds to at most 448, so saturation never acts and the codes are torch's x.to(float8_e4m3fn) of the same fp32 product.
+template <int kMaxVec>
+__device__ __forceinline__ float row_amax(const Vec8 (&v)[kMaxVec], int nvec, int lane) {
+  float m = 0.f;
+#pragma unroll
+  for (int i = 0; i < kMaxVec; ++i)
+    if (lane + i * 32 < nvec) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float2 f = e2_to_float2(v[i].h[j]);
+        m = fmaxf(m, fmaxf(fabsf(f.x), fabsf(f.y)));
+      }
+    }
+  return warp_max(m);
+}
+
+template <int kMaxVec>
+__device__ __forceinline__ void store_row_e4m3(const Vec8 (&v)[kMaxVec], int nvec, int lane, float amax, uint8_t* qrow,
+                                               float* scale) {
+  const float s = amax > 0.f ? __fdiv_rn(448.f, amax) : 0.f;
+#pragma unroll
+  for (int i = 0; i < kMaxVec; ++i) {
+    const int vi = lane + i * 32;
+    if (vi < nvec) {
+      uint32_t w[2] = {0u, 0u};
+      if (amax > 0.f) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const float2 f = e2_to_float2(v[i].h[j]);
+          const uint32_t c = __nv_cvt_float2_to_fp8x2(make_float2(f.x * s, f.y * s), __NV_SATFINITE, __NV_E4M3);
+          w[j >> 1] |= c << (16 * (j & 1));
+        }
+      }
+      *reinterpret_cast<uint2*>(qrow + vi * 8) = make_uint2(w[0], w[1]);
+    }
+  }
+  if (lane == 0) *scale = amax > 0.f ? __fdiv_rn(amax, 448.f) : 1.f;
+}
+
+// [rows, C] 16-bit -> e4m3 codes + per-row scales, a warp per row (C <= kMaxVec * 256)
+template <int kMaxVec>
+__global__ void __launch_bounds__(256) quant_rows_fp8_kernel(const bf16* __restrict__ x, uint8_t* __restrict__ q,
+                                                             float* __restrict__ scale, int C, long long rows) {
+  const int lane = threadIdx.x & 31;
+  const int nvec = C >> 3;
+  const long long stride = (long long)gridDim.x * (blockDim.x >> 5);
+  for (long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); row < rows; row += stride) {
+    Vec8 v[kMaxVec];
+    const bf16* xr = x + (size_t)row * C;
+#pragma unroll
+    for (int i = 0; i < kMaxVec; ++i)
+      if (lane + i * 32 < nvec) v[i].u = ld_stream(xr + (lane + i * 32) * 8);
+    store_row_e4m3<kMaxVec>(v, nvec, lane, row_amax<kMaxVec>(v, nvec, lane), q + (size_t)row * C, scale + row);
+  }
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // LayerNorm (no affine) + modulate + per-frame select.  One warp per token row; the row lives in registers.
 // kMaxVec: max 16-byte vectors per lane (C <= kMaxVec*32*8).
@@ -48,14 +114,17 @@ struct LnDspArgs {
 
 // kMinBlocks: resident 256-thread blocks per SM the register budget is sized for; 3 at hidden <= 1280 = 80 registers,
 // 24 resident warps per SM (one 2.3 KB row in flight each).
-template <int kMaxVec, bool kDsp, int kMinBlocks>
+// kFp8: instead of the 16-bit row, store its e4m3 codes to q and its scale to qscale (store_row_e4m3 over the 16-bit
+// outputs, so the result is that of vsb_quant_rows_fp8 on the 16-bit output).
+template <int kMaxVec, bool kDsp, int kMinBlocks, bool kFp8 = false>
 __global__ void __launch_bounds__(256, kMinBlocks) ln_modulate_kernel(const bf16* __restrict__ x, bf16* __restrict__ out,
                                                           const bf16* __restrict__ mod,
                                                           const uint8_t* __restrict__ x_mask, int shift_row,
                                                           int scale_row, int B, int T, int S, int C, float eps,
                                                           long long rows, const bf16* __restrict__ gamma,
                                                           const bf16* __restrict__ beta,
-                                                          const __grid_constant__ LnDspArgs dsp) {
+                                                          const __grid_constant__ LnDspArgs dsp,
+                                                          uint8_t* __restrict__ q, float* __restrict__ qscale) {
   const int warps_per_block = blockDim.x >> 5;
   const int lane = threadIdx.x & 31;
   const int nvec = C >> 3;
@@ -140,9 +209,13 @@ __global__ void __launch_bounds__(256, kMinBlocks) ln_modulate_kernel(const bf16
           const elem2 g2 = __hadd2_rn(one2, sc.h[j]);
           o.h[j] = __hadd2_rn(__hmul2_rn(n2, g2), sh.h[j]);
         }
-        if (!kDsp || send) st_stream(orow + vi * 8, o.u);
+        if (kFp8)
+          v[i].u = o.u;
+        else if (!kDsp || send)
+          st_stream(orow + vi * 8, o.u);
       }
     }
+    if (kFp8) store_row_e4m3<kMaxVec>(v, nvec, lane, row_amax<kMaxVec>(v, nvec, lane), q + (size_t)row * C, qscale + row);
   }
   if (kDsp) {
     // zero rows of the padded frames [B*T, Tl*world): the receiver's attention reads them (the reference pads zeros)
@@ -475,12 +548,15 @@ static int grid_for(long long work_items, int per_block) {
 
 using namespace vsb;
 
+// q != null: the e4m3 output (codes q, per-row scales qscale) instead of out; never with dsp or gamma / beta
 static int ln_modulate_launch(const vsb_bf16* x, vsb_bf16* out, const vsb_bf16* mod, const uint8_t* x_mask,
                               const vsb_bf16* gamma, const vsb_bf16* beta, int shift_row, int scale_row, int B, int T,
-                              int S, int C, float eps, const LnDspArgs* dsp, void* stream) {
+                              int S, int C, float eps, const LnDspArgs* dsp, void* stream, uint8_t* q = nullptr,
+                              float* qscale = nullptr) {
   if ((gamma == nullptr) != (beta == nullptr)) return fail(VSB_ERR_INVALID, "ln_modulate: gamma and beta go together");
-  if (!x || (!out && !dsp) || !mod || B <= 0 || T <= 0 || S <= 0 || C <= 0) return fail(VSB_ERR_INVALID, "ln_modulate: bad args");
-  if (C % 8 || C > 3072 || (dsp && C > 2048) || !aligned16(x) || !aligned16(out) || !aligned16(mod))
+  if (!x || (!out && !dsp && !q) || !mod || B <= 0 || T <= 0 || S <= 0 || C <= 0) return fail(VSB_ERR_INVALID, "ln_modulate: bad args");
+  if (q != nullptr && (qscale == nullptr || dsp || gamma)) return fail(VSB_ERR_INVALID, "ln_modulate_fp8: bad args");
+  if (C % 8 || C > 3072 || (dsp && C > 2048) || !aligned16(x) || !aligned16(out) || !aligned16(mod) || !aligned16(q))
     return fail(VSB_ERR_UNSUPPORTED, "ln_modulate: need C %% 8 == 0, C <= 3072 (2048 with the fused reshard), 16B-aligned pointers (C=%d)", C);
   if (shift_row < 0 || shift_row > 5 || scale_row < 0 || scale_row > 5) return fail(VSB_ERR_INVALID, "ln_modulate: row");
   long long rows = (long long)B * T * S;
@@ -489,11 +565,17 @@ static int ln_modulate_launch(const vsb_bf16* x, vsb_bf16* out, const vsb_bf16* 
   cudaStream_t st = (cudaStream_t)stream;
   LnDspArgs none;
   memset(&none, 0, sizeof(none));
-#define VSB_LN_LAUNCH(MV, DSP, OCC, ARGS)                                                                              \
-  ln_modulate_kernel<MV, DSP, OCC><<<grid, 256, 0, st>>>((const bf16*)x, (bf16*)out, (const bf16*)mod, x_mask,         \
-                                                          shift_row, scale_row, B, T, S, C, eps, rows,                  \
-                                                          (const bf16*)gamma, (const bf16*)beta, ARGS)
-  if (dsp) {
+#define VSB_LN_LAUNCH(MV, DSP, OCC, ARGS, ...)                                                                         \
+  ln_modulate_kernel<MV, DSP, OCC, ##__VA_ARGS__><<<grid, 256, 0, st>>>((const bf16*)x, (bf16*)out, (const bf16*)mod,   \
+                                                                         x_mask, shift_row, scale_row, B, T, S, C, eps, \
+                                                                         rows, (const bf16*)gamma, (const bf16*)beta,   \
+                                                                         ARGS, q, qscale)
+  if (q != nullptr) {
+    if (C <= 1280) VSB_LN_LAUNCH(5, false, 3, none, true);
+    else if (C <= 2048) VSB_LN_LAUNCH(8, false, 2, none, true);
+    else if (C <= 2304) VSB_LN_LAUNCH(9, false, 2, none, true);
+    else VSB_LN_LAUNCH(12, false, 1, none, true);
+  } else if (dsp) {
     if (C <= 1280) VSB_LN_LAUNCH(5, true, 3, *dsp); else VSB_LN_LAUNCH(8, true, 2, *dsp);
   } else if (C <= 1280) {
     VSB_LN_LAUNCH(5, false, 3, none);
@@ -568,6 +650,27 @@ extern "C" int vsb_gate_residual_dsp(const vsb_bf16* x, void* const* host_peer_y
 extern "C" int VSB_API(vsb_ln_modulate)(const vsb_bf16* x, vsb_bf16* out, const vsb_bf16* mod, const uint8_t* x_mask,
                                int shift_row, int scale_row, int B, int T, int S, int C, float eps, void* stream) {
   return VSB_API(vsb_ln_modulate_affine)(x, out, mod, x_mask, nullptr, nullptr, shift_row, scale_row, B, T, S, C, eps, stream);
+}
+
+extern "C" int VSB_API(vsb_ln_modulate_fp8)(const vsb_bf16* x, uint8_t* q, float* scale, const vsb_bf16* mod,
+                                            const uint8_t* x_mask, int shift_row, int scale_row, int B, int T, int S, int C,
+                                            float eps, void* stream) {
+  if (!q) return fail(VSB_ERR_INVALID, "ln_modulate_fp8: bad args");
+  return ln_modulate_launch(x, nullptr, mod, x_mask, nullptr, nullptr, shift_row, scale_row, B, T, S, C, eps, nullptr, stream,
+                            q, scale);
+}
+
+extern "C" int VSB_API(vsb_quant_rows_fp8)(const vsb_bf16* x, uint8_t* q, float* scale, int M, int K, void* stream) {
+  if (!x || !q || !scale || M <= 0 || K <= 0) return fail(VSB_ERR_INVALID, "quant_rows_fp8: bad args");
+  if (K % 8 || K > 4608 || !aligned16(x) || !aligned16(q))
+    return fail(VSB_ERR_UNSUPPORTED, "quant_rows_fp8: need K %% 8 == 0, K <= 4608, 16B-aligned pointers (K=%d)", K);
+  const int grid = grid_for(M, 8);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (K <= 1280)
+    quant_rows_fp8_kernel<5><<<grid, 256, 0, st>>>((const bf16*)x, q, scale, K, M);
+  else
+    quant_rows_fp8_kernel<18><<<grid, 256, 0, st>>>((const bf16*)x, q, scale, K, M);
+  return check_launch("quant_rows_fp8");
 }
 
 extern "C" int VSB_API(vsb_modulation_table)(const vsb_bf16* table, const vsb_bf16* t, const vsb_bf16* t0, vsb_bf16* mod,

@@ -21,6 +21,11 @@
 // A consumer releases a stage once the wgmma that read it has retired, and its staging tile once the TMA store has read
 // it (cp.async.bulk.wait_group.read).  TMA zero-fills K/M/N tails on load and clips them on store, so any M,
 // N % 8 == 0, K % 8 == 0 is legal.
+//
+// e4m3 operands (vsb_gemm_fp8_*): gemm_wide_kernel on WideFp8Cfg, 128 x 128 tiles, k-blocks of 128 elements -- the same
+// 128-byte swizzled rows, so the producer, the stage ring and the descriptors are those of the 16-bit kernels -- with
+// wgmma.m64n128k32.e4m3 and each k-block's products promoted into fp32 registers (consumer_k_loop), and y =
+// bf16(acc * sa[row] * sw[col] + bias) at the start of the shared epilogue.  K % 16 == 0 (16-byte rows of codes).
 #include "vsb_common.cuh"
 #include "vsb_host.h"
 #include "wgmma.cuh"
@@ -35,9 +40,10 @@ constexpr int kPersistentGeluMaxK = 1536;  // longest K at which a GELU epilogue
 constexpr long long kWideMinTiles = 2048;  // fewest 256 x 128 tiles at which gemm_route picks gemm_wide_kernel
 
 // Each kernel's tile, launch and shared memory.  kStageBytes: the A boxes then the W box of one k-block.
+// kBK: elements of K per k-block (one 128-byte swizzle row); kFp8: e4m3 operands.
 struct GemmCfg {  // gemm_wgmma_kernel
-  static constexpr int kTileM = kBM, kTileN = kBN;
-  static constexpr bool kPersistent = true;
+  static constexpr int kTileM = kBM, kTileN = kBN, kBK = vsb::kBK;
+  static constexpr bool kPersistent = true, kFp8 = false;
   // two consumer warpgroups + one producer warp; ptxas allots 168 registers per thread: 128 accumulators + the epilogue
   static constexpr int kThreads = 288;
   static constexpr int kABytes = kABox;
@@ -50,8 +56,8 @@ struct GemmCfg {  // gemm_wgmma_kernel
 
 template <int BN>
 struct TileCfg {  // gemm_tile_kernel<BN, .>
-  static constexpr int kTileM = kBM, kTileN = BN;
-  static constexpr bool kPersistent = false;
+  static constexpr int kTileM = kBM, kTileN = BN, kBK = vsb::kBK;
+  static constexpr bool kPersistent = false, kFp8 = false;
   static constexpr int kThreads = 384;
   static constexpr int kABytes = kABox;
   static constexpr int kStageBytes = (kBM + BN) * kBK * 2;
@@ -62,17 +68,25 @@ struct TileCfg {  // gemm_tile_kernel<BN, .>
 };
 
 constexpr int kWideEpiThreads = 96;
-struct WideCfg {  // gemm_wide_kernel
-  static constexpr int kTileM = 2 * kBM, kTileN = kBN;
-  static constexpr bool kPersistent = true;
+// gemm_wide_kernel.  16-bit operands: 256 x 128 tiles, each consumer warpgroup 128 rows.  e4m3 operands (FP8 = true):
+// 128 x 128 tiles, each consumer 64 rows -- the fp32 promotion fragment doubles the accumulators, and 2 x 64 of them
+// per thread fit the 168-register budget where 2 x 128 would not; a k-block is 128 elements, the same 128-byte rows.
+template <bool FP8>
+struct WideCfgT {
+  static constexpr int kTileM = FP8 ? kBM : 2 * kBM, kTileN = kBN, kBK = FP8 ? 128 : vsb::kBK;
+  static constexpr bool kPersistent = true, kFp8 = FP8;
   static constexpr int kThreads = 384;  // two consumer warpgroups, three epilogue warps, one producer warp
-  static constexpr int kABytes = 2 * kABox;  // two 128-row TMA boxes
-  static constexpr int kStageBytes = kABytes + kBN * kBK * 2;
-  static constexpr int kCBytes = kBM * kBN * 2;  // one consumer's half of the staging tile
-  static constexpr int kStages = 3;
-  // 3 x 48 KB ring + 2 x 32 KB staging, + 1024 for manual alignment, + 256 for barriers: 214 272 B of the 227 KB
-  static constexpr int kSmemBytes = kStages * kStageBytes + 2 * kCBytes + 1024 + 256;
+  static constexpr int kCBlocks = kTileM / kBM;  // 128-row TMA boxes of A, and of the staging tile
+  static constexpr int kABytes = kCBlocks * kABox;
+  static constexpr int kStageBytes = kABytes + kBN * 128;
+  static constexpr int kCBytes = kBM * kBN * 2;  // one 128-row block of the staging tile
+  static constexpr int kStages = FP8 ? 6 : 3;
+  // 16-bit: 3 x 48 KB ring + 2 x 32 KB staging; e4m3: 6 x 32 KB ring + 32 KB staging; + 1024 for manual alignment, + 256
+  // for barriers: 214 272 / 230 656 B of the 227 KB
+  static constexpr int kSmemBytes = kStages * kStageBytes + kCBlocks * kCBytes + 1024 + 256;
 };
+using WideCfg = WideCfgT<false>;
+using WideFp8Cfg = WideCfgT<true>;
 
 // ---- the epilogue's element functions: every kernel applies them to y = bf16(acc + bias), two adjacent columns -------
 __device__ __forceinline__ float gelu_tanh_f(float x) {
@@ -104,6 +118,8 @@ struct EpiArgs {
   const bf16* mod;        // [2, B, 6, N] or null
   const uint8_t* x_mask;  // [B, T] or null
   int gate_row, B, T, S;
+  const float* sa;        // e4m3 operands: per-row scale of A [M] and per-output-channel scale of W [N]
+  const float* sw;
 };
 
 // element offset in mod of output row `row`'s gate vector: row gate_row of its sample's t (or, where x_mask marks the
@@ -130,7 +146,8 @@ __device__ __forceinline__ float2 residual_add2(float2 y, uint32_t resid, bool g
 // acc[hm] holds rows 64 hm .. 64 hm + 63 of the block whose first output element is (m0, n0); the 16-bit result goes
 // to the consumer's 128B-swizzled staging rows at my_c ([BN/64][128 rows][128 B]), for the caller to TMA-store.  ACT 2
 // reads resid from the same slots, where the producer's TMA load lands it (resid_full completes phase `parity`).
-template <int BN, int HALVES, int ACT>
+// FP8: acc sums e4m3 products, y = bf16(fmaf(acc * sa[row], sw[col], bias[col])) (ep.sa, ep.sw).
+template <int BN, int HALVES, int ACT, bool FP8 = false>
 __device__ __forceinline__ void gemm_epilogue(const float (&acc)[HALVES][BN / 2], uint32_t my_c, int m0, int n0, int M,
                                               int N, const bf16* __restrict__ bias, const EpiArgs& ep,
                                               uint64_t* resid_full, uint32_t parity, int warp, int lane) {
@@ -140,6 +157,7 @@ __device__ __forceinline__ void gemm_epilogue(const float (&acc)[HALVES][BN / 2]
   const int rl = warp * 16 + (lane >> 2);
   const uint32_t c_row = my_c + rl * 128 + (lane & 3) * 4;
   int gate_off[HALVES][2];  // element offset of the row's gate vector in mod, -1: none
+  float row_scale[HALVES][2];  // FP8: sa of the row
 #pragma unroll
   for (int hm = 0; hm < HALVES; ++hm)
 #pragma unroll
@@ -147,6 +165,8 @@ __device__ __forceinline__ void gemm_epilogue(const float (&acc)[HALVES][BN / 2]
       const int grow = m0 + rl + 8 * h + 64 * hm;
       gate_off[hm][h] = -1;
       if (ACT == 2 && ep.gate_row >= 0 && grow < M) gate_off[hm][h] = gate_offset(ep, grow, N);
+      row_scale[hm][h] = 0.f;
+      if (FP8 && grow < M) row_scale[hm][h] = __ldg(ep.sa + grow);
     }
   if (ACT == 2) mbar_wait_quiet(resid_full, parity);  // the resid block is in the staging tile
 #pragma unroll
@@ -155,6 +175,8 @@ __device__ __forceinline__ void gemm_epilogue(const float (&acc)[HALVES][BN / 2]
     const int gcol = n0 + col;
     float2 b2 = make_float2(0.f, 0.f);
     if (bias != nullptr && gcol < N) b2 = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(bias + gcol)));
+    float2 sw2 = make_float2(0.f, 0.f);
+    if (FP8 && gcol < N) sw2 = __ldg(reinterpret_cast<const float2*>(ep.sw + gcol));
 #pragma unroll
     for (int hm = 0; hm < HALVES; ++hm)
 #pragma unroll
@@ -162,6 +184,9 @@ __device__ __forceinline__ void gemm_epilogue(const float (&acc)[HALVES][BN / 2]
         const int row = rl + 8 * h + 64 * hm;
         const uint32_t dst = c_row + (jj >> 3) * (kBM * 128) + (8 * h + 64 * hm) * 128 + (((jj & 7) ^ (rl & 7)) << 4);
         float2 x = make_float2(acc[hm][4 * jj + 2 * h] + b2.x, acc[hm][4 * jj + 2 * h + 1] + b2.y);
+        if (FP8)
+          x = make_float2(fmaf(acc[hm][4 * jj + 2 * h] * row_scale[hm][h], sw2.x, b2.x),
+                          fmaf(acc[hm][4 * jj + 2 * h + 1] * row_scale[hm][h], sw2.y, b2.y));
         if (ACT == 1) x = gelu2<1>(make_float2(rbf(x.x), rbf(x.y)));
         if (ACT == 2 && m0 + row < M && gcol < N) {
           const bool gated = gate_off[hm][h] >= 0;
@@ -198,9 +223,9 @@ __device__ __forceinline__ void load_k_block(const CUtensorMap* tm_a, const CUte
   mbar_wait_quiet(&empty[s], ((n / Cfg::kStages) & 1) ^ 1);
   unsigned char* sa = smem_ab + s * Cfg::kStageBytes;
   mbar_arrive_expect_tx(&full[s], a_boxes * kABox + Cfg::kStageBytes - Cfg::kABytes);
-  tma_load_2d(tm_a, &full[s], sa, kb * kBK, m0);
-  if (a_boxes == 2) tma_load_2d(tm_a, &full[s], sa + kABox, kb * kBK, m0 + kBM);
-  tma_load_2d(tm_w, &full[s], sa + Cfg::kABytes, kb * kBK, n0);
+  tma_load_2d(tm_a, &full[s], sa, kb * Cfg::kBK, m0);
+  if (a_boxes == 2) tma_load_2d(tm_a, &full[s], sa + kABox, kb * Cfg::kBK, m0 + kBM);
+  tma_load_2d(tm_w, &full[s], sa + Cfg::kABytes, kb * Cfg::kBK, n0);
 }
 
 template <int BN>
@@ -214,6 +239,9 @@ __device__ __forceinline__ void wgmma_tile(float (&d)[BN / 2], uint64_t da, uint
 // One consumer's K loop over the k-blocks at ring positions n_base .. n_base + num_kb - 1: per k16 step one
 // wgmma.m64n{BN}k16 per 64-row half, A from a_off inside the stage.  Each stage is released once the wgmma that read
 // it has retired, all but the last: the caller releases that after its wgmma_wait<0>.
+// e4m3 (Cfg::kFp8): per k32 step one wgmma.m64n128k32.e4m3, and each k-block's chain of four runs into a fresh
+// fragment that is then added to the fp32 accumulators (promotion every 128 of K: the tensor core's own accumulation
+// of fp8 products keeps fewer bits than fp32, so it never sums more than one k-block).
 template <class Cfg, int HALVES>
 __device__ __forceinline__ void consumer_k_loop(float (&acc)[HALVES][Cfg::kTileN / 2], uint32_t ab0, uint32_t a_off,
                                                 uint64_t* full, uint64_t* empty, int n_base, int num_kb, int t) {
@@ -221,6 +249,32 @@ __device__ __forceinline__ void consumer_k_loop(float (&acc)[HALVES][Cfg::kTileN
   for (int hm = 0; hm < HALVES; ++hm)
 #pragma unroll
     for (int i = 0; i < Cfg::kTileN / 2; ++i) acc[hm][i] = 0.f;
+  if constexpr (Cfg::kFp8) {
+    static_assert(Cfg::kTileN == 128, "the e4m3 K loop runs m64n128k32");
+    float part[HALVES][Cfg::kTileN / 2];
+    for (int kb = 0; kb < num_kb; ++kb) {
+      const int n = n_base + kb, s = n % Cfg::kStages;
+      mbar_wait_quiet(&full[s], (n / Cfg::kStages) & 1);
+      const uint32_t sa = ab0 + s * Cfg::kStageBytes + a_off;
+      const uint32_t sw = ab0 + s * Cfg::kStageBytes + Cfg::kABytes;
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const uint64_t dw = wgmma_desc_sw128(sw + 32 * k);
+#pragma unroll
+        for (int hm = 0; hm < HALVES; ++hm)
+          wgmma_m64n128k32_e4m3_ss(part[hm], wgmma_desc_sw128(sa + hm * (64 * 128) + 32 * k), dw, k > 0 ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      if (kb > 0 && t == 0) mbar_arrive(&empty[(n - 1) % Cfg::kStages]);
+#pragma unroll
+      for (int hm = 0; hm < HALVES; ++hm)
+#pragma unroll
+        for (int i = 0; i < Cfg::kTileN / 2; ++i) acc[hm][i] += part[hm][i];
+    }
+    return;
+  }
   for (int kb = 0; kb < num_kb; ++kb) {
     const int n = n_base + kb, s = n % Cfg::kStages;
     mbar_wait_quiet(&full[s], (n / Cfg::kStages) & 1);
@@ -416,28 +470,31 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
 // gemm_epilogue) and go on to the next tile's mainloop; three epilogue warps then apply the rest in place -- tanh-GELU(y),
 // erf-GELU(y), or resid + [bf16(gate * y)] with resid read from global memory -- and TMA-store the tile.
 // Every step sees the same 16-bit y and calls the same element functions as gemm_wgmma_kernel, so the outputs are
-// bit-identical.  Barriers per staging half c: st_full[c] (the consumer's 128 threads have written y), st_free[c] (the
-// tile's TMA store has read the half).
-template <int ACT>
-__global__ void __launch_bounds__(WideCfg::kThreads, 1)
+// bit-identical.  Barriers per consumer c: st_full[c] (the consumer's 128 threads have written y), st_free[c] (the
+// tile's TMA store has read the consumer's rows).
+// With e4m3 operands (WideFp8Cfg) the tile is 128 x 128, each consumer owns 64 rows of it, and y is
+// bf16(acc * sa * sw + bias) (gemm_epilogue); the epilogue warps and their element functions are the same.
+template <class Cfg, int ACT>
+__global__ void __launch_bounds__(Cfg::kThreads, 1)
 gemm_wide_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_w,
                  const __grid_constant__ CUtensorMap tm_c, const __grid_constant__ CUtensorMap tm_r,
                  const bf16* __restrict__ bias, int M, int N, int K, const EpiArgs ep) {
-  using Cfg = WideCfg;
   constexpr int kStages = Cfg::kStages;
+  constexpr int kRowsC = Cfg::kTileM / 2;     // rows of a tile per consumer
+  constexpr int kHalves = kRowsC / 64;        // 64-row wgmma halves per consumer
   extern __shared__ unsigned char smem_dyn[];
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~uintptr_t(1023));
-  unsigned char* smem_ab = smem;                              // [kStages][A 32 KB | W 16 KB]
-  unsigned char* smem_c = smem + kStages * Cfg::kStageBytes;  // [consumer][kBN/64][128 rows][128 B] swizzled
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem_c + 2 * Cfg::kCBytes);  // [kStages]
-  uint64_t* empty = full + kStages;                                         // [kStages]
+  unsigned char* smem_ab = smem;                              // [kStages][A 32 / 16 KB | W 16 KB]
+  unsigned char* smem_c = smem + kStages * Cfg::kStageBytes;  // [kCBlocks][kBN/64][128 rows][128 B] swizzled
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem_c + Cfg::kCBlocks * Cfg::kCBytes);  // [kStages]
+  uint64_t* empty = full + kStages;                                                      // [kStages]
   uint64_t* st_full = empty + kStages;  // [2]
   uint64_t* st_free = st_full + 2;      // [2]
 
   const int wg = threadIdx.x >> 7;
   const int tiles_n = (N + kBN - 1) / kBN;
   const int tiles = ((M + Cfg::kTileM - 1) / Cfg::kTileM) * tiles_n;
-  const int num_kb = (K + kBK - 1) / kBK;
+  const int num_kb = (K + Cfg::kBK - 1) / Cfg::kBK;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tm_a);
@@ -461,7 +518,7 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant
       int n = 0;  // k-blocks loaded so far: the position in the ring, carried over between tiles
       for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
         const int m0 = (tile / tiles_n) * Cfg::kTileM, n0 = (tile % tiles_n) * kBN;
-        const int a_boxes = m0 + kBM < M ? 2 : 1;  // the lower half's A box only where it has rows inside M
+        const int a_boxes = Cfg::kCBlocks == 2 && m0 + kBM < M ? 2 : 1;  // the lower box only where it has rows inside M
         for (int kb = 0; kb < num_kb; ++kb, ++n) load_k_block<Cfg>(&tm_a, &tm_w, smem_ab, full, empty, n, kb, m0, n0, a_boxes);
       }
     } else if (threadIdx.x < 256 + kWideEpiThreads) {
@@ -477,7 +534,7 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant
           // 16-byte unit u of the staging tile = 8 columns of one row: u = ((half * 2 + chunk) * 128 + row) * 8 + slot,
           // the slot holding column group slot ^ (row & 7) of the 128B swizzle
 #pragma unroll 2
-          for (int u = e; u < 2 * Cfg::kCBytes / 16; u += kWideEpiThreads) {
+          for (int u = e; u < Cfg::kCBlocks * Cfg::kCBytes / 16; u += kWideEpiThreads) {
             const int row = (u >> 3) & (kBM - 1), hc = u >> 10;
             const int grow = m0 + (hc >> 1) * kBM + row;
             const int gcol = n0 + (hc & 1) * 64 + (((u & 7) ^ (row & 7)) << 3);
@@ -513,7 +570,7 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant
         named_bar_sync(1, kWideEpiThreads);
         if (e == 0) {
 #pragma unroll 1
-          for (int h = 0; h < 2; ++h)
+          for (int h = 0; h < Cfg::kCBlocks; ++h)
             for (int ch = 0; ch < kBN / 64; ++ch)
               if (m0 + h * kBM < M && n0 + ch * 64 < N)
                 tma_store_2d_s(&tm_c, c0 + h * Cfg::kCBytes + ch * (kBM * 128), n0 + ch * 64, m0 + h * kBM);
@@ -528,35 +585,39 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant
     return;
   }
 
-  // ===================== consumers: warpgroup c takes rows 128 c .. 128 c + 127 of every tile of the CTA ==============
+  // ===================== consumers: warpgroup c takes rows kRowsC c .. kRowsC c + kRowsC - 1 of every tile ============
   const int c = wg;
   const int t = threadIdx.x & 127;
   const int warp = t >> 5, lane = t & 31;
-  const uint32_t my_c = smem_u32(smem_c) + c * Cfg::kCBytes;
+  // the consumer's first row in the staging tile: 128-row block c (16-bit), or row 64 c of the one block (e4m3)
+  const uint32_t my_c = smem_u32(smem_c) + c * (kRowsC == kBM ? Cfg::kCBytes : kRowsC * 128);
   const uint32_t ab0 = smem_u32(smem_ab);
   int j = 0;
   for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x, ++j) {
-    const int m0 = (tile / tiles_n) * Cfg::kTileM + c * kBM, n0 = (tile % tiles_n) * kBN;
-    float acc[2][64];
+    const int m0 = (tile / tiles_n) * Cfg::kTileM + c * kRowsC, n0 = (tile % tiles_n) * kBN;
+    float acc[kHalves][64];
     const int n_base = j * num_kb;  // ring position of this tile's first k-block
-    consumer_k_loop<Cfg, 2>(acc, ab0, c * kABox, full, empty, n_base, num_kb, t);
+    consumer_k_loop<Cfg, kHalves>(acc, ab0, c * kRowsC * 128, full, empty, n_base, num_kb, t);
     wgmma_wait<0>();
     if (t == 0) mbar_arrive(&empty[(n_base + num_kb - 1) % kStages]);
 
-    if (j > 0) mbar_wait_quiet(&st_free[c], (j - 1) & 1);  // the previous tile's store has read this half
-    gemm_epilogue<kBN, 2, 0>(acc, my_c, m0, n0, M, N, bias, ep, nullptr, 0, warp, lane);  // y = bf16(acc + bias)
+    if (j > 0) mbar_wait_quiet(&st_free[c], (j - 1) & 1);  // the previous tile's store has read these rows
+    // y = bf16(acc + bias), or bf16(acc * sa * sw + bias)
+    gemm_epilogue<kBN, kHalves, 0, Cfg::kFp8>(acc, my_c, m0, n0, M, N, bias, ep, nullptr, 0, warp, lane);
     fence_proxy_async_smem();  // bias only: the TMA store reads y as written
     mbar_arrive(&st_full[c]);
   }
 }
 
 // ---- host side ---------------------------------------------------------------------------------------------------------
-// Tensor map of a row-major [rows, cols] 16-bit matrix, moved in 128B-swizzled boxes of box_rows x 64 columns.
-static int make_tmap_rows(CUtensorMap* m, const void* p, int rows, int cols, int box_rows) {
+// Tensor map of a row-major [rows, cols] 16-bit (or, fp8, 1-byte) matrix, moved in 128B-swizzled boxes of box_rows
+// rows x 128 bytes.
+static int make_tmap_rows(CUtensorMap* m, const void* p, int rows, int cols, int box_rows, bool fp8 = false) {
+  const int esize = fp8 ? 1 : 2;
   const unsigned long long dims[2] = {(unsigned long long)cols, (unsigned long long)rows};
-  const unsigned long long stride[1] = {(unsigned long long)cols * 2};
-  const unsigned box[2] = {64, (unsigned)box_rows};
-  return make_tmap_bf16(m, p, 2, dims, stride, box, CU_TENSOR_MAP_SWIZZLE_128B);
+  const unsigned long long stride[1] = {(unsigned long long)cols * esize};
+  const unsigned box[2] = {128u / esize, (unsigned)box_rows};
+  return make_tmap_elem(fp8 ? kTmapDtypeU8 : VSB_TMAP_DTYPE, m, p, 2, dims, stride, box, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
 typedef int (*GemmLaunch)(const void* A, const void* W, const bf16* bias, void* out, int M, int N, int K,
@@ -575,8 +636,8 @@ static int launch_gemm(const void* A, const void* W, const bf16* bias, void* out
     attr = true;
   }
   CUtensorMap ta, tw, tc, tr;
-  int rc = make_tmap_rows(&ta, A, M, K, kBM);
-  if (!rc) rc = make_tmap_rows(&tw, W, N, K, Cfg::kTileN);
+  int rc = make_tmap_rows(&ta, A, M, K, kBM, Cfg::kFp8);
+  if (!rc) rc = make_tmap_rows(&tw, W, N, K, Cfg::kTileN, Cfg::kFp8);
   if (!rc) rc = make_tmap_rows(&tc, out, M, N, kBM);
   if (rc) return rc;
   tr = tc;  // unused without a resid
@@ -611,10 +672,16 @@ static const GemmInstance kGemmInstances[4][4] = {
      {launch_gemm<gemm_wgmma_kernel<1>, GemmCfg>, "gemm_wgmma_kernel<1>"},
      {launch_gemm<gemm_wgmma_kernel<2>, GemmCfg>, "gemm_wgmma_kernel<2>"},
      {launch_gemm<gemm_wgmma_kernel<3>, GemmCfg>, "gemm_wgmma_kernel<3>"}},
-    {{launch_gemm<gemm_wide_kernel<0>, WideCfg>, "gemm_wide_kernel<0>"},
-     {launch_gemm<gemm_wide_kernel<1>, WideCfg>, "gemm_wide_kernel<1>"},
-     {launch_gemm<gemm_wide_kernel<2>, WideCfg>, "gemm_wide_kernel<2>"},
-     {launch_gemm<gemm_wide_kernel<3>, WideCfg>, "gemm_wide_kernel<3>"}}};
+    {{launch_gemm<gemm_wide_kernel<WideCfg, 0>, WideCfg>, "gemm_wide_kernel<0>"},
+     {launch_gemm<gemm_wide_kernel<WideCfg, 1>, WideCfg>, "gemm_wide_kernel<1>"},
+     {launch_gemm<gemm_wide_kernel<WideCfg, 2>, WideCfg>, "gemm_wide_kernel<2>"},
+     {launch_gemm<gemm_wide_kernel<WideCfg, 3>, WideCfg>, "gemm_wide_kernel<3>"}}};
+
+// The e4m3 instances by epilogue (0 none, 1 tanh-GELU, 2 fused residual): gemm_route_fp8 picks one for every shape.
+static const GemmInstance kGemmFp8Instances[3] = {
+    {launch_gemm<gemm_wide_kernel<WideFp8Cfg, 0>, WideFp8Cfg>, "gemm_wide_kernel<fp8, 0>"},
+    {launch_gemm<gemm_wide_kernel<WideFp8Cfg, 1>, WideFp8Cfg>, "gemm_wide_kernel<fp8, 1>"},
+    {launch_gemm<gemm_wide_kernel<WideFp8Cfg, 2>, WideFp8Cfg>, "gemm_wide_kernel<fp8, 2>"}};
 
 // Which kernel runs a GEMM; act: 0 none, 1 tanh-GELU, 2 fused residual, 3 erf-GELU.
 static GemmKernel gemm_route(int M, int N, int K, int act) {
@@ -652,6 +719,23 @@ static int gemm_dispatch(const void* A, const void* W, const void* bias, void* o
   return g.launch(A, W, (const bf16*)bias, out, M, N, K, ep, st);
 }
 
+// Which e4m3 instance runs a GEMM; act: 0 none, 1 tanh-GELU, 2 fused residual.  Every shape takes the persistent
+// 128 x 128 kernel: the promotion fragment rules out the 256-row tile, and no epilogue is left on the tensor cores' path.
+static const GemmInstance& gemm_route_fp8(int act) { return kGemmFp8Instances[act]; }
+
+static int gemm_fp8_dispatch(const void* A, const float* sa, const void* W, const float* sw, const void* bias, void* out,
+                             int M, int N, int K, int act, cudaStream_t st, EpiArgs ep) {
+  if (!A || !sa || !W || !sw || !out || M <= 0 || N <= 0 || K <= 0) return fail(VSB_ERR_INVALID, "gemm_fp8: bad args");
+  if (K % 16 || N % 8 || !aligned16(A) || !aligned16(W) || !aligned16(out) || !aligned16(sw) ||
+      (ep.resid != nullptr && !aligned16(ep.resid)))
+    return fail(VSB_ERR_UNSUPPORTED, "gemm_fp8: need K %% 16 == 0, N %% 8 == 0, 16B-aligned pointers (M=%d N=%d K=%d)", M, N, K);
+  if ((long long)((M + kBM - 1) / kBM) * ((N + kBN - 1) / kBN) > 0x7fffffffLL)
+    return fail(VSB_ERR_UNSUPPORTED, "gemm_fp8: too many tiles (M=%d N=%d)", M, N);
+  ep.sa = sa;
+  ep.sw = sw;
+  return gemm_route_fp8(act).launch(A, W, (const bf16*)bias, out, M, N, K, ep, st);
+}
+
 }  // namespace vsb
 
 using namespace vsb;
@@ -681,7 +765,33 @@ extern "C" int VSB_API(vsb_gemm_bias_residual)(const vsb_bf16* A, const vsb_bf16
   return gemm_dispatch(A, W, bias, out, M, N, K, 2, (cudaStream_t)stream, ep);
 }
 
+// e4m3 operands, see include/vsb200.h: out = act(bf16(acc * sa[m] * sw[n] + bias)).
+extern "C" int VSB_API(vsb_gemm_fp8_bias_act)(const uint8_t* A, const float* sa, const uint8_t* W, const float* sw,
+                                              const vsb_bf16* bias, vsb_bf16* out, int M, int N, int K, int act, void* stream) {
+  if (act < 0 || act > 1) return fail(VSB_ERR_INVALID, "gemm_fp8: act=%d", act);
+  return gemm_fp8_dispatch(A, sa, W, sw, bias, out, M, N, K, act, (cudaStream_t)stream, EpiArgs{nullptr, nullptr, nullptr, -1, 1, 1, 1});
+}
+
+extern "C" int VSB_API(vsb_gemm_fp8_bias_residual)(const uint8_t* A, const float* sa, const uint8_t* W, const float* sw,
+                                                   const vsb_bf16* bias, const vsb_bf16* resid, vsb_bf16* out,
+                                                   const vsb_bf16* mod, const uint8_t* x_mask, int gate_row, int M, int N,
+                                                   int K, int B, int T, int S, void* stream) {
+  if (!resid) return fail(VSB_ERR_INVALID, "gemm_fp8_residual: bad args");
+  if (gate_row >= 0) {
+    if (!mod || gate_row > 5 || B <= 0 || T <= 0 || S <= 0 || (long long)B * T * S != M || !aligned16(mod))
+      return fail(VSB_ERR_INVALID, "gemm_fp8_residual: gate needs mod[2,B,6,N] and B*T*S == M");
+  }
+  EpiArgs ep{(const bf16*)resid, (const bf16*)mod, x_mask, gate_row, B, T, S};
+  return gemm_fp8_dispatch(A, sa, W, sw, bias, out, M, N, K, 2, (cudaStream_t)stream, ep);
+}
+
 #ifndef VSB_HALF
+// The kernel gemm_fp8_dispatch picks for a shape (the same for both 16-bit output types), see include/vsb200.h.
+extern "C" const char* vsb_gemm_fp8_kernel_name(int M, int N, int K, int act, int residual) {
+  if (M <= 0 || N <= 0 || K <= 0 || act < 0 || act > 1 || (residual && act != 0)) return "";
+  return gemm_route_fp8(residual ? 2 : act).name;
+}
+
 // The kernel gemm_dispatch picks for a shape (the same for both 16-bit types), see include/vsb200.h.
 extern "C" const char* vsb_gemm_kernel_name(int M, int N, int K, int act, int residual) {
   if (M <= 0 || N <= 0 || K <= 0 || act < 0 || act > 2 || (residual && act != 0)) return "";

@@ -35,13 +35,14 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 EncodeTiledFn encode_tiled();
 
-// 16-bit tensor map (dtype 0 = bf16, 1 = fp16), rank <= 5; dims/strides innermost first; strides in BYTES for dims
+// Tensor map (dtype 0 = bf16, 1 = fp16, kTmapDtypeU8 = 1-byte), rank <= 5; dims/strides innermost first; strides in BYTES for dims
 // 1..rank-1.  elem_strides (null: all 1) are TMA traversal strides: dimension i loads box[i] / elem_strides[i] elements,
 // every elem_strides[i]-th one.  Cached by (dtype, base, shape, strides, box, traversal strides, swizzle).
 int make_tmap_elem(int dtype, CUtensorMap* m, const void* base, int rank, const unsigned long long* dims,
                    const unsigned long long* strides_bytes, const unsigned* box, CUtensorMapSwizzle swz,
                    const unsigned* elem_strides = nullptr);
 int num_sms();
+constexpr int kTmapDtypeU8 = 2;  // make_tmap_elem dtype of 1-byte elements (e4m3 codes)
 }  // namespace vsbs
 
 #ifndef VSB_TMAP_DTYPE

@@ -565,6 +565,84 @@ def gemm_kernel_name(M: int, N: int, K: int, act: int = 0, residual: bool = Fals
     return name
 
 
+def _fp8_codes(t, name):
+    if t.dtype not in (torch.float8_e4m3fn, torch.uint8):
+        raise _lib.VsbError(f"{name} must hold e4m3 codes (float8_e4m3fn or uint8), got {t.dtype}")
+
+
+def quant_rows_fp8(x):
+    """(q, scale): e4m3 codes [..., K] (float8_e4m3fn) and fp32 per-row scales [...] of x [..., K], by the rule of
+    include/vsb200.h (scale = amax / 448 of the row, 1 for an all-zero row)."""
+    lib, st = _prep(x)
+    _bf16(x, "x")
+    K = x.shape[-1]
+    M = x.numel() // K
+    q = torch.empty(x.shape, dtype=torch.float8_e4m3fn, device=x.device)
+    scale = torch.empty(x.shape[:-1], dtype=torch.float32, device=x.device)
+    with _Timed("quant", 3 * M * K + 4 * M):
+        _lib.check(_fn(lib, "vsb_quant_rows_fp8", x)(_p(x), _p(q), _p(scale), M, K, st), "quant_rows_fp8")
+    return q, scale
+
+
+def ln_modulate_fp8(x, mod, x_mask_u8, shift_row, scale_row, B, T, S, eps=1e-6):
+    """ln_modulate with its output quantized: (q, scale) == quant_rows_fp8(ln_modulate(...)) bit for bit."""
+    lib, st = _prep(x, mod, x_mask_u8)
+    _bf16(x, "x")
+    _same_dtype(x, mod)
+    Cc = x.shape[-1]
+    rows = x.numel() // Cc
+    q = torch.empty(x.shape, dtype=torch.float8_e4m3fn, device=x.device)
+    scale = torch.empty(x.shape[:-1], dtype=torch.float32, device=x.device)
+    with _Timed("ln_modulate", 3 * x.numel() + 4 * rows):
+        _lib.check(_fn(lib, "vsb_ln_modulate_fp8", x)(_p(x), _p(q), _p(scale), _p(mod), _p(x_mask_u8), shift_row, scale_row, B, T,
+                                                      S, Cc, eps, st), "ln_modulate_fp8")
+    return q, scale
+
+
+def gemm_fp8_bias_act(a, a_scale, w, w_scale, bias=None, act: int = 0, out=None, dtype=torch.bfloat16):
+    """out[..., N] = act(bf16(acc * a_scale[m] * w_scale[n] + bias)) with a [..., K], w [N, K] e4m3 codes; out in bias's
+    16-bit dtype (else dtype)."""
+    lib, st = _prep(a, a_scale, w, w_scale, bias, out)
+    _fp8_codes(a, "a"), _fp8_codes(w, "w"), _bf16(bias, "bias")
+    K = a.shape[-1]
+    M = a.numel() // K
+    N = w.shape[0]
+    if w.shape[1] != K:
+        raise _lib.VsbError("gemm_fp8: K mismatch")
+    ref = bias if bias is not None else (out if out is not None else torch.empty(0, dtype=dtype))
+    _same_dtype(bias, out)
+    out = torch.empty(*a.shape[:-1], N, dtype=ref.dtype, device=a.device) if out is None else out
+    with _Timed("gemm_fp8", 2 * M * N * K):
+        _lib.check(_fn(lib, "vsb_gemm_fp8_bias_act", ref)(_p(a), _p(a_scale), _p(w), _p(w_scale), _p(bias), _p(out), M, N, K, act,
+                                                          st), "gemm_fp8_bias_act")
+    return out
+
+
+def gemm_fp8_bias_residual(a, a_scale, w, w_scale, bias, resid, mod=None, x_mask_u8=None, gate_row: int = -1, B=1, T=1, S=1,
+                           out=None):
+    """out = resid + [gate *] bf16(acc * a_scale * w_scale + bias), fused as gemm_bias_residual (out defaults to resid)."""
+    lib, st = _prep(a, a_scale, w, w_scale, bias, resid, mod, x_mask_u8, out)
+    _fp8_codes(a, "a"), _fp8_codes(w, "w"), _bf16(resid, "resid")
+    _same_dtype(bias, resid, mod, out)
+    K = a.shape[-1]
+    M = a.numel() // K
+    N = w.shape[0]
+    out = resid if out is None else out
+    with _Timed("gemm_fp8", 2 * M * N * K):
+        _lib.check(_fn(lib, "vsb_gemm_fp8_bias_residual", resid)(_p(a), _p(a_scale), _p(w), _p(w_scale), _p(bias), _p(resid), _p(out),
+                                                                 _p(mod), _p(x_mask_u8), gate_row, M, N, K, B, T, S, st),
+                   "gemm_fp8_bias_residual")
+    return out
+
+
+def gemm_fp8_kernel_name(M: int, N: int, K: int, act: int = 0, residual: bool = False) -> str:
+    """The kernel instance gemm_fp8_bias_act (act) or gemm_fp8_bias_residual (residual=True) launches."""
+    name = _lib.load().vsb_gemm_fp8_kernel_name(M, N, K, act, int(residual)).decode()
+    if not name:
+        raise _lib.VsbError(f"gemm_fp8_kernel_name: bad arguments M={M} N={N} K={K} act={act} residual={residual}")
+    return name
+
+
 def attn_flash(q, k, v, nb, nq, nk, H, D, q_row_stride, q_batch_stride, kv_row_stride, kv_batch_stride, scale,
                kv_lens: Optional[Sequence[int]] = None, out=None, out_row_stride=None, out_batch_stride=None):
     """q/k/v: tensors whose data_ptr() is the first element of the strided view (may be slices of one buffer).

@@ -194,6 +194,7 @@ class STDiT3(nn.Module):
         self._text_cache = None  # per (y, mask): caption MLP output, key layout, per-block kv_linear outputs
         self._hw_cache = None
         self._final_pad = None
+        self._fp8 = False
 
     # ------------------------------------------------------------------------------------------------------
     def initialize_weights(self):
@@ -223,6 +224,62 @@ class STDiT3(nn.Module):
         self.parallel_manager = parallel_mgr if parallel_mgr is not None else parallel_manager(dp_size, sp_size, enable_cp)
         for blk in [*self.spatial_blocks, *self.temporal_blocks]:
             blk.parallel_manager = self.parallel_manager
+
+    # ---- FP8 Linears (opt-in) ----------------------------------------------------------------------------------------
+    # The block Linears that run on the e4m3 GEMM in FP8 mode: the two whose input the modulate kernel quantizes as it
+    # writes it.  The other four need a quantization pass of their own, and with it they lose to the bf16 kernel at
+    # 720p (bench_gemm.py, H100 80GB HBM3, 700 W, SM clock 1980 MHz; DESIGN.md section 9): attn.proj 1.51 against
+    # 0.76 ms, q_linear 0.66 / 0.57, cross_attn.proj 1.44 / 0.71, fc2 2.39 / 2.33 ms, where qkv (1.35 / 1.65 ms) and
+    # fc1 (2.08 / 2.37 ms) win.  kv_linear (once per prompt), the embedders, t_block, the final layer and all attention
+    # stay bf16 too.
+    FP8_LINEARS = (("attn", "qkv"), ("mlp", "fc1"))
+
+    def _fp8_modules(self):
+        for blk in [*self.spatial_blocks, *self.temporal_blocks]:
+            for owner, name in self.FP8_LINEARS:
+                yield getattr(getattr(blk, owner), name)
+
+    @staticmethod
+    def _fp8_refresh(lin: nn.Linear):
+        """(Re)quantizes lin's weight into its non-persistent buffers fp8_weight (e4m3 codes, uint8 so that a dtype
+        conversion of the module leaves them alone) and fp8_scale (fp32 per output channel) unless they were taken from
+        the current parameter: the key follows load_state_dict (the in-place copy bumps _version) and .to() (new
+        storage), and a conversion of the scale buffer's dtype is caught by its own check."""
+        w = lin.weight
+        key = (w.data_ptr(), w._version, w.dtype, w.device)
+        sc = lin._buffers.get("fp8_scale")
+        if getattr(lin, "_fp8_key", None) == key and sc is not None and sc.dtype == torch.float32 and sc.device == w.device:
+            return
+        q, scale = kernels.quant_rows_fp8(w.detach())
+        lin.register_buffer("fp8_weight", q.view(torch.uint8), persistent=False)
+        lin.register_buffer("fp8_scale", scale, persistent=False)
+        lin._fp8_key = key
+
+    def set_fp8_linears(self, enabled: bool):
+        """FP8 mode: the block Linears FP8_LINEARS of every block run on e4m3 operands -- weights quantized per output
+        channel, activations per token row (include/vsb200.h) -- with fp32 accumulation.  Results differ from the
+        bf16 path by the quantization.  Disabling restores the bf16 calls exactly.  One GPU only (sp == 1)."""
+        pm = self.parallel_manager
+        if enabled and pm is not None and pm.sp_size > 1:
+            raise NotImplementedError("FP8 Linears under sequence parallelism (the fused DSP modulate would need an fp8 push)")
+        self._fp8 = bool(enabled)
+        for lin in self._fp8_modules():
+            if not enabled:
+                for name in ("fp8_weight", "fp8_scale"):
+                    lin._buffers.pop(name, None)
+                lin._fp8_key = None
+            elif lin.weight.is_cuda:  # otherwise at the first forward, once the model is on the GPU
+                self._fp8_refresh(lin)
+        return self
+
+    def _ln_gemm(self, lin, x, mod, mask_u8, shift_row, scale_row, B, T, S, act=0):
+        """lin(ln_modulate(x)) [tanh-GELU]: in FP8 mode the modulate kernel emits the e4m3 rows and their scales, and the
+        e4m3 GEMM takes them."""
+        if self._fp8:
+            qa, sa = kernels.ln_modulate_fp8(x, mod, mask_u8, shift_row, scale_row, B, T, S)
+            return kernels.gemm_fp8_bias_act(qa, sa, lin.fp8_weight, lin.fp8_scale, lin.bias, act)
+        return kernels.gemm_bias_act(kernels.ln_modulate(x, mod, mask_u8, shift_row, scale_row, B, T, S), lin.weight, lin.bias,
+                                     act=act)
 
     def reset_pab_state(self, drop_caches: bool = False):
         for blk in [*self.spatial_blocks, *self.temporal_blocks]:
@@ -376,8 +433,7 @@ class STDiT3(nn.Module):
             if wq is None:
                 raise RuntimeError("vsb200 STDiT3 kernels implement qk_norm=True (the OpenSora v1.2 configuration)")
             if blk.temporal:
-                xm = K.ln_modulate(x, mod, mask_u8, 0, 1, B, T, S)
-                qkv = K.gemm_bias_act(xm, a.qkv.weight, a.qkv.bias)
+                qkv = self._ln_gemm(a.qkv, x, mod, mask_u8, 0, 1, B, T, S)
                 # T < 30: native_attention semantics in one kernel (attentions.py:95-97,111-120); T >= 30: the reference
                 # takes F.scaled_dot_product_attention (attentions.py:98-100), same softmax on the flash kernel
                 o = temporal_attention(qkv, B, T, S, H, D, D**-0.5, 29, wq, wk, rope=self._rope_tables(T, x.device))
@@ -397,9 +453,11 @@ class STDiT3(nn.Module):
                     Ta, Sa = xm.shape[1], xm.shape[2]
                     xm = xm.reshape(Ba, Ta * Sa, C)
                 else:
-                    xm = K.ln_modulate(x, mod, mask_u8, 0, 1, B, T, S)
                     Ta, Sa = T, S
-                qkv = K.gemm_bias_act(xm, a.qkv.weight, a.qkv.bias)
+                if sp > 1:
+                    qkv = K.gemm_bias_act(xm, a.qkv.weight, a.qkv.bias)
+                else:
+                    qkv = self._ln_gemm(a.qkv, x, mod, mask_u8, 0, 1, B, T, S)
                 o = packed_self_attention(qkv, Ba * Ta, Sa, H, D, D**-0.5, short_max=29, wq=wq, wk=wk)
             cache = None
             if pab_on:
@@ -439,8 +497,7 @@ class STDiT3(nn.Module):
                 K.residual_add(x, blk.last_cross.view(x.shape), out=x)
 
         # ---- MLP ----
-        xm = K.ln_modulate(x, mod, mask_u8, 3, 4, B, T, S)
-        h = K.gemm_bias_act(xm, blk.mlp.fc1.weight, blk.mlp.fc1.bias, act=1)
+        h = self._ln_gemm(blk.mlp.fc1, x, mod, mask_u8, 3, 4, B, T, S, act=1)
         K.gemm_bias_residual(h.view(-1, h.shape[-1]), blk.mlp.fc2.weight, blk.mlp.fc2.bias, x, mod, mask_u8, 5, B, T, S)
         return x
 
@@ -470,6 +527,11 @@ class STDiT3(nn.Module):
         T, Hn, Wn = self.get_dynamic_size(x)
         B = x.size(0)
         C = self.hidden_size
+        if self._fp8:
+            if sp > 1:
+                raise NotImplementedError("FP8 Linears under sequence parallelism (the fused DSP modulate would need an fp8 push)")
+            for lin in self._fp8_modules():
+                self._fp8_refresh(lin)
         if sp > 1 and Tx == 1:
             raise NotImplementedError("image mode (one frame) under sequence parallelism: the reference scatters the "
                                       "batch instead (:292-296); run images on one GPU")

@@ -94,7 +94,7 @@ class OpenSoraConfig:
                  enable_flash_attn: bool = False, enable_pab: bool = False, pab_config=None,
                  transformer_config: Optional[STDiT3Config] = None, state_dict=None,
                  text_encoder_fn: Optional[Callable] = None, vae_decode_fn: Optional[Callable] = None,
-                 vae_encoder=None):
+                 vae_encoder=None, fp8_linears: bool = False):
         self.pipeline_cls = OpenSoraPipeline
         # vae: a local snapshot directory of hpcai-tech/OpenSora-VAE-v1.2 or a VideoAutoencoderPipeline instance decodes
         # natively; anything else (the default hub id) leaves generate() returning latents
@@ -115,6 +115,8 @@ class OpenSoraConfig:
         self.state_dict = state_dict
         self.text_encoder_fn = text_encoder_fn
         self.vae_decode_fn = vae_decode_fn
+        # FP8 mode of the denoiser (STDiT3.set_fp8_linears): the six block Linears on e4m3 operands; off keeps the bf16 path
+        self.fp8_linears = fp8_linears
 
 
 @dataclass
@@ -139,6 +141,8 @@ class OpenSoraPipeline:
         if config.state_dict is not None:
             self.transformer.load_state_dict(config.state_dict)
         self.transformer = self.transformer.to(self._device).eval()
+        if config.fp8_linears:
+            self.transformer.set_fp8_linears(True)
         self.scheduler = RFLOW(num_sampling_steps=config.num_sampling_steps, cfg_scale=config.cfg_scale,
                                use_timestep_transform=True)
         self.vae = self._load_vae()
