@@ -17,6 +17,11 @@ Axes name the dimensions of the output: ``b`` sample, ``t`` frame, ``n`` token (
 and columns of a latent, flatten row-major into one token index), ``c`` channel.  A missing letter is an axis of extent 1.
 Golden files of large cases keep a seeded sample of the output elements and their flat index; ``idx`` / ``shape`` take
 that form, and the sampled elements are grouped by (sample, frame) only.
+
+Image-shaped outputs (decoded video, latents) name their pixel rows ``h`` and columns ``w`` instead of ``n``: their slices
+are then 2-D tiles of TILE_HW x TILE_HW pixels (partial at the far edges) by 128 channels, all channels when fewer than
+128.  A 64 x 64 RGB tile holds 12 288 elements, about as many as a 128 x 128 slice.  Row-major token tiles would be bands
+across the whole width, in which an error along one vertical seam (a tiled decoder's blend zone) is a small fraction.
 """
 import math
 from dataclasses import dataclass
@@ -25,6 +30,7 @@ from typing import Optional, Sequence
 import torch
 
 TILE = 128
+TILE_HW = 64  # pixel rows and columns of a 2-D tile
 K = 1.25
 FLOOR = 0.25
 OLD_K = 1.25  # the whole-output gate: ||ours - r32|| <= OLD_K * ||r16 - r32|| + 1e-4 ||r32||
@@ -33,11 +39,11 @@ OLD_K = 1.25  # the whole-output gate: ||ours - r32|| <= OLD_K * ||r16 - r32|| +
 @dataclass
 class SliceReport:
     name: str
-    grid: tuple  # slices per axis: (samples, frames, token tiles, channel tiles)
-    tile: tuple  # (token rows, channels) per slice
+    grid: tuple  # slices per axis: (samples, frames, token tiles, channel tiles); 2-D: (.., row tiles, column tiles, ..)
+    tile: tuple  # (token rows, channels) per slice; 2-D: (pixel rows, pixel columns, channels)
     loads: torch.Tensor  # [grid] err_s / bound_s
     ratios: torch.Tensor  # [grid] err_s / ref_s
-    worst_at: tuple  # (sample, frame, first token, first channel) of the worst slice
+    worst_at: tuple  # (sample, frame, first token, first channel) of the worst slice; 2-D: (.., first row, first column, ..)
     worst_err: float
     worst_ref: float
     floor: float
@@ -56,9 +62,14 @@ class SliceReport:
         q = torch.tensor([0.5, 0.9, 0.99, 1.0], dtype=torch.float64)
         lq = torch.quantile(self.loads.flatten(), q).tolist()
         rq = torch.quantile(self.ratios.flatten().clamp(max=1e6), q).tolist()
-        b, t, n, c = self.worst_at
-        return (f"[slices] {self.name}: {self.loads.numel()} slices {self.grid} of {self.tile[0]} tokens x {self.tile[1]} channels; "
-                f"worst load {self.worst:.3f} at sample {b} frame {t} tokens {n}.. channels {c}.. "
+        if len(self.tile) == 3:
+            b, t, y, x, c = self.worst_at
+            shape, where = f"{self.tile[0]} x {self.tile[1]} pixels x {self.tile[2]} channels", f"rows {y}.. columns {x}.."
+        else:
+            b, t, n, c = self.worst_at
+            shape, where = f"{self.tile[0]} tokens x {self.tile[1]} channels", f"tokens {n}.."
+        return (f"[slices] {self.name}: {self.loads.numel()} slices {self.grid} of {shape}; "
+                f"worst load {self.worst:.3f} at sample {b} frame {t} {where} channels {c}.. "
                 f"(err {self.worst_err:.3e}, own 16-bit err {self.worst_ref:.3e}, floor {self.floor:.3e}); "
                 f"load p50/p90/p99/max {lq[0]:.3f}/{lq[1]:.3f}/{lq[2]:.3f}/{lq[3]:.3f}; "
                 f"err/own p50/p90/p99/max {rq[0]:.3f}/{rq[1]:.3f}/{rq[2]:.3f}/{rq[3]:.3f}; "
@@ -89,11 +100,34 @@ def _tile_sq(d: torch.Tensor, tn: int, tc: int) -> torch.Tensor:
     return d.view(B, T, nt, tn, ct, tc).sum(dim=(3, 5))
 
 
+def _canon_hw(t: torch.Tensor, axes: str) -> torch.Tensor:
+    """t as float64 [B, T, H, W, C] for axes naming one ``h`` and one ``w`` dimension and no ``n``."""
+    if len(axes) != t.dim() or set(axes) - set("bthwc") or axes.count("h") != 1 or axes.count("w") != 1:
+        raise ValueError(f"axes {axes!r} must name each of the {t.dim()} dimensions with one of b, t, h, w, c (h and w once)")
+    perm = [i for a in "bthwc" for i, x in enumerate(axes) if x == a]
+    ext = tuple(math.prod(s for a, s in zip(axes, t.shape) if a == x) for x in "bthwc")
+    return t.double().permute(perm).reshape(ext)
+
+
+def _tile_sq_hw(d: torch.Tensor, th: int, tw: int, tc: int) -> torch.Tensor:
+    """Per-tile sums of squares of d [B, T, H, W, C]: [B, T, ceil(H/th), ceil(W/tw), ceil(C/tc)]."""
+    B, T, H, W, C = d.shape
+    nh, nw, nc = -(-H // th), -(-W // tw), -(-C // tc)
+    d = torch.nn.functional.pad(d * d, (0, nc * tc - C, 0, nw * tw - W, 0, nh * th - H))
+    return d.view(B, T, nh, th, nw, tw, nc, tc).sum(dim=(3, 5, 7))
+
+
 def sliced_parity(name: str, ours, r16, r32, axes: str, idx: Optional[torch.Tensor] = None,
                   shape: Optional[Sequence[int]] = None, k: float = K, floor: float = FLOOR) -> SliceReport:
     """The rule on full outputs of the shape the axes describe, or, with idx and shape, on the elements idx (flat indices
     into an output of that shape) of it: ours / r16 / r32 then hold those elements in the order of idx."""
-    if idx is None:
+    if idx is None and "h" in axes:
+        o, a, r = (_canon_hw(x, axes) for x in (ours, r16, r32))
+        assert o.shape == a.shape == r.shape, (ours.shape, r16.shape, r32.shape)
+        tile = (TILE_HW, TILE_HW, min(o.shape[-1], TILE))
+        err2, ref2 = _tile_sq_hw(o - r, *tile), _tile_sq_hw(a - r, *tile)
+        tot_r, tot_e = r.norm().item(), (o - r).norm().item()
+    elif idx is None:
         o, a, r = (_canon(x, axes) for x in (ours, r16, r32))
         assert o.shape == a.shape == r.shape, (ours.shape, r16.shape, r32.shape)
         B, T, N, C = o.shape
@@ -101,6 +135,7 @@ def sliced_parity(name: str, ours, r16, r32, axes: str, idx: Optional[torch.Tens
         # holds about TILE x TILE elements: a norm over 128 elements scatters by tens of per cent on its own
         tn, tc = (TILE, TILE) if C >= TILE else (TILE * -(-TILE // C), C)
         err2, ref2 = _tile_sq(o - r, tn, tc), _tile_sq(a - r, tn, tc)
+        tile = (tn, tc)
         tot_r, tot_e = r.norm().item(), (o - r).norm().item()
     else:
         shape = tuple(shape)
@@ -113,7 +148,7 @@ def sliced_parity(name: str, ours, r16, r32, axes: str, idx: Optional[torch.Tens
             for i, x in enumerate(axes):
                 if x == letter:
                     bt = bt * shape[i] + coord[i]
-        tn, tc = N, C
+        tile = (N, C)
         err2 = torch.zeros(B * T, dtype=torch.float64).index_add_(0, bt, (o - r) ** 2).view(B, T, 1, 1)
         ref2 = torch.zeros(B * T, dtype=torch.float64).index_add_(0, bt, (a - r) ** 2).view(B, T, 1, 1)
         tot_r, tot_e = r.norm().item(), (o - r).norm().item()
@@ -123,9 +158,9 @@ def sliced_parity(name: str, ours, r16, r32, axes: str, idx: Optional[torch.Tens
     loads = err / (k * ref + fl)
     ratios = err / ref.clamp_min(1e-300)
     w = int(loads.flatten().argmax())
-    b, t, i, j = torch.unravel_index(torch.tensor(w), loads.shape)
-    return SliceReport(name=name, grid=tuple(loads.shape), tile=(tn, tc), loads=loads, ratios=ratios,
-                       worst_at=(int(b), int(t), int(i) * tn, int(j) * tc), worst_err=err.flatten()[w].item(),
+    at = torch.unravel_index(torch.tensor(w), loads.shape)
+    return SliceReport(name=name, grid=tuple(loads.shape), tile=tile, loads=loads.cpu(), ratios=ratios.cpu(),
+                       worst_at=tuple(int(i) * s for i, s in zip(at, (1, 1) + tile)), worst_err=err.flatten()[w].item(),
                        worst_ref=ref.flatten()[w].item(), floor=fl, whole_ratio=tot_e / max(tot_ref, 1e-300),
                        old_gate_ok=tot_e <= OLD_K * tot_ref + 1e-4 * tot_r)
 
@@ -134,6 +169,5 @@ def assert_sliced_parity(name: str, ours, r16, r32, axes: str, **kw) -> SliceRep
     """sliced_parity, printed, and asserted."""
     rep = sliced_parity(name, ours, r16, r32, axes, **kw)
     print(rep.describe())
-    assert rep.ok, (f"{name}: slice at sample {rep.worst_at[0]} frame {rep.worst_at[1]} tokens {rep.worst_at[2]}.. "
-                    f"channels {rep.worst_at[3]}.. is {rep.worst:.3f}x its bound")
+    assert rep.ok, f"{name}: slice at (sample, frame, ..) {rep.worst_at} is {rep.worst:.3f}x its bound"
     return rep
